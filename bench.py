@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- predict_instances throughput of the B200 path (and of the reference CPU path).
+"""bench.py -- predict_instances throughput of the H100 path (and of the reference CPU path).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (one rank per GPU under torchrun)
   python bench.py --impl reference --steps K --warmup W     # the reference's CPU path (oracle)
+  python bench.py ... --dump-outputs DIR                    # also write the last timed step's outputs as DIR/<name>.npy
 
 One JSON line.  What it holds (BASELINE.json: "instances/sec (predict_instances end-to-end) 2D 1024^2 r=32 & 3D 128x512^2 r=96"):
 
@@ -11,12 +12,18 @@ One JSON line.  What it holds (BASELINE.json: "instances/sec (predict_instances 
                                 in HBM; `e2e` = host image in -> host labels + polygons out through the public API.
                                 N > 1: every rank processes its own copy of the image (weak scaling, no data-path collective).
   value_3d / e2e_3d / roofline_3d   configs[2]: StarDist3D.predict_instances on a 128x512x512 volume, Rays_GoldenSpiral(96),
-                                default Config3D; same two timings (fewer steps, stated in config.steps_3d).
-  big_2d / big_3d               configs[3] / [4]: predict_instances_big on a tiled 8192x8192 image / a 512^3 anisotropic volume,
+                                default Config3D; same two timings, K timed steps.
+  big_2d / big_3d               (--big) configs[3] / [4]: predict_instances_big on a tiled 8192x8192 image / a 512^3 anisotropic volume,
                                 blocks sharded over the N ranks (strong scaling: the image is fixed, value = instances of the
                                 whole image / max-over-ranks wall time incl. the device-to-device tile gather and the D2H of
                                 the assembled label map on rank 0).
-  cpu_baseline                  the reference's CPU path timed on this box's host cores (see --impl reference).
+  cpu_baseline                  (--cpu-baseline) the reference's CPU path timed on this box's host cores (see --impl reference).
+  device                        name and power limit of the GPU the numbers were measured on.
+
+--dump-outputs DIR writes what the timed device path (predict_instances_device) returned in its last timed step, float32 /
+float64 .npy files: labels_2d, points_2d, prob_2d, coord_2d; with the 3-D workload points_3d, prob_3d, dist_3d and
+labels_sample_3d (the label volume at a fixed, seeded sample of voxels, labels_sample_index_3d = their flat indices).
+The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse, json, os, sys, time, threading, subprocess
 import numpy as np
@@ -38,6 +45,37 @@ REF_SAMPLE_3D = (64, 256, 256)     # CPU arms time one eighth of the 3-D volume 
 METRIC = "instances/sec (predict_instances end-to-end)"
 W2D = "StarDist2D predict_instances, 1024x1024, n_rays=32, seeded synthetic U-Net weights (configs[1])"
 W3D = "StarDist3D predict_instances, 128x512x512, Rays_GoldenSpiral n_rays=96, seeded synthetic U-Net weights (configs[2])"
+DUMP_3D_VOXELS = 1 << 21           # sampled voxels of the 3-D label volume written by --dump-outputs (8 MB as float32)
+
+
+def gpu_info(index=0):
+    """name and power limit of the measuring GPU (both are part of every number the benchmark reports)"""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=10).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": int(out[2])}
+    except Exception as e:
+        return {"error": repr(e)[:200]}
+
+
+def dump_outputs(dirname, suffix, labels, res, label_sample=None):
+    """the arrays predict_instances_device returned, as float32 / float64 .npy files (labels: all of them in 2-D, a fixed
+    seeded sample of voxels in 3-D)"""
+    os.makedirs(dirname, exist_ok=True)
+    host = lambda a: np.asarray(a.cpu().numpy() if hasattr(a, "cpu") else a)
+    arrays = {}
+    lab = host(labels)
+    if label_sample is None:
+        arrays["labels"] = lab.astype(np.float32)
+    else:
+        idx = np.sort(np.random.default_rng(0).choice(lab.size, size=min(label_sample, lab.size), replace=False))
+        arrays["labels_sample"] = lab.reshape(-1)[idx].astype(np.float32)
+        arrays["labels_sample_index"] = idx.astype(np.float64)
+    for k in ("points", "prob", "coord", "dist"):
+        if k in res:
+            arrays[k] = host(res[k]).astype(np.float32)
+    for k, a in arrays.items():
+        np.save(os.path.join(dirname, "%s_%s.npy" % (k, suffix)), a)
 
 
 class ClockSampler(threading.Thread):
@@ -161,13 +199,13 @@ def reference_numbers(steps, warmup, budget_s=240.0):
         except Exception as e:
             tried[t] = 0.0
     best_t = max(tried, key=tried.get)
-    r2 = _run_worker(2, best_t, max(1, min(steps, 5)), min(1, warmup))
+    r2 = _run_worker(2, best_t, steps, min(1, warmup))
     out = {"threads_sweep_2d_instances_per_s": {str(k): v for k, v in tried.items()}, "best_threads": best_t, "cores": cores,
            "value_2d": r2["instances"] / r2["seconds"], "ms_per_step_2d": 1000 * r2["seconds"] / r2["steps"], "steps_2d": r2["steps"],
            "stages_ms_2d": r2["stages_ms"]}
     try:
         t3 = best_t
-        r3 = _run_worker(3, t3, max(1, min(steps, 2)), 0 if time.perf_counter() - t_start > 0.5 * budget_s else 1)
+        r3 = _run_worker(3, t3, steps, 0 if time.perf_counter() - t_start > 0.5 * budget_s else 1)
         out.update({"value_3d": r3["instances"] / r3["seconds"], "ms_per_step_3d": 1000 * r3["seconds"] / r3["steps"], "steps_3d": r3["steps"],
                     "stages_ms_3d": r3["stages_ms"], "threads_3d": t3})
     except Exception as e:
@@ -205,16 +243,19 @@ def run_reference(args):
     }))
 
 
-# ====================================================================================== B200 arm
+# ====================================================================================== GPU arm
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200")
-    ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--skip-3d", action="store_true")
-    ap.add_argument("--skip-big", action="store_true")
+    # the two extra workloads take minutes at K steps (a 512^3 big pass ~8 s, a CPU 3-D step ~13 s): run on request
+    ap.add_argument("--big", action="store_true", help="also time predict_instances_big (configs[3] / [4]), K passes each")
+    ap.add_argument("--cpu-baseline", action="store_true", help="also time the reference's CPU path on the host cores, K steps")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, < 64 MB)")
     ap.add_argument("--dim", type=int, default=2)          # reference-worker only
     ap.add_argument("--threads", type=int, default=8)      # reference-worker only
     args = ap.parse_args()
@@ -237,7 +278,7 @@ def main():
         _lib.load().sdb_nms3d_set_variant(int(os.environ["STARDIST_B200_NMS3D_VARIANT"]))
     if os.environ.get("STARDIST_B200_NMS2D_TAIL"):
         _lib.load().sdb_nms2d_set_tail(int(os.environ["STARDIST_B200_NMS2D_TAIL"]))
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 50 MB L2
 
     def barrier():
         if world > 1: dist.barrier()
@@ -254,7 +295,7 @@ def main():
 
     def time_device(model, x_dev, shape, pthr, nthr, steps):
         """device-resident timing: CUDA events around predict_instances_device, L2 flushed between steps"""
-        n_inst = 0; dev_ms = 0.0; stage = {}; n_cand = 0
+        n_inst = 0; dev_ms = 0.0; stage = {}; n_cand = 0; last = None
         for _ in range(steps):
             flush.zero_()
             model._events = []
@@ -262,11 +303,12 @@ def main():
             e0.record()
             labels, res = model.predict_instances_device(x_dev, shape, prob_thresh=pthr, nms_thresh=nthr)
             e1.record(); torch.cuda.synchronize()
+            last = (labels, res)
             dev_ms += e0.elapsed_time(e1); n_inst += len(res['prob']); n_cand += getattr(model, '_last_n_cand', 0)
             ev = dict(model._events); model._events = None
             for a, b, k in STAGES:
                 if a in ev and b in ev: stage[k] = stage.get(k, 0.0) + ev[a].elapsed_time(ev[b])
-        return dev_ms, n_inst, n_cand, stage
+        return dev_ms, n_inst, n_cand, stage, last
 
     def time_e2e(model, img, pthr, nthr, steps, warmup=2):
         model._stats = {}
@@ -287,14 +329,11 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak_tf_burst = peaks.get("bf16_tflops", 1700.0)
-    peak_tf_sust = peaks.get("bf16_tflops_sustained", 1400.0)
-    peak_bw = peaks.get("hbm_gbs", 6650.0)
-    src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        traffic = {}
+    # fallback: NVIDIA's H100 SXM data sheet (dense FP16/BF16 tensor rate, HBM3 bandwidth; 700 W part)
+    peak_tf_burst = peaks.get("bf16_tflops", 989.0)
+    peak_tf_sust = peaks.get("bf16_tflops_sustained", peak_tf_burst)
+    peak_bw = peaks.get("hbm_gbs", 3350.0)
+    src = "MEASURED_PEAKS.json" if peaks else "fallback (H100 SXM data sheet, not measured)"
 
     # ------------------------------------------------------------------ configs[1]: 2-D 1024^2
     cfg = Config2D(n_rays=N_RAYS)
@@ -307,7 +346,10 @@ def main():
     _lib.launch_count(reset=True)
     _lib.profile_enable(True)
     barrier()
-    dev_ms, n_inst, n_cand, stage = time_device(model, x_dev, SHAPE, PROB_THRESH, NMS_THRESH, args.steps)
+    dev_ms, n_inst, n_cand, stage, last = time_device(model, x_dev, SHAPE, PROB_THRESH, NMS_THRESH, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, "2d", *last)
+    del last
     launches = _lib.launch_count()
     prof_conv = _lib.profile_get("conv_tc")
     prof_nms = {k: _lib.profile_get("nms2d_" + k) for k in ("frontier", "pairs", "fast", "clip", "tail")}
@@ -325,21 +367,18 @@ def main():
         pairs_per_step = prof_nms["fast"]["units"] / args.steps if prof_nms["fast"]["units"] else 0.0
         conv_ms = prof_conv["ms"]
         ach = prof_conv["units"] / (conv_ms / 1e3) / 1e12 if conv_ms > 0 else 0.0
-        roof = {"name": "conv_tc", "bound": "tensor", "kernel": "k_conv_tc* (tcgen05 3x3 convolutions + fused 1x1 heads, all launches of the forward pass)",
+        roof = {"name": "conv_tc", "bound": "tensor", "kernel": "k_conv_wg (wgmma 3x3 convolutions + fused 1x1 heads, all launches of the forward pass)",
                 "achieved": ach, "peak": peak_tf_burst, "unit": "TFLOP/s", "frac": ach / peak_tf_burst, "frac_of_sustained_peak": ach / peak_tf_sust,
-                "traffic": None, "ms_per_step": conv_ms / args.steps, "launches_per_step": prof_conv["launches"] / args.steps,
+                "ms_per_step": conv_ms / args.steps, "launches_per_step": prof_conv["launches"] / args.steps,
                 "algorithmic_flop_per_step": prof_conv["units"] / args.steps, "issued_flop_factor": 3, "unet_forward_ms": unet_ms,
                 "unet_algorithmic_tflops": fl / (unet_ms / 1e3) / 1e12 if unet_ms > 0 else None,
                 "peak_source": src + " bf16_tflops (burst: a ~1 ms kernel group timed alone)"}
-        if "conv_tc" in traffic and roof["launches_per_step"]:
-            roof["traffic"] = traffic["conv_tc"]["dram_bytes_per_step"] / roof["launches_per_step"]; roof["traffic_source"] = traffic["conv_tc"]["source"]
         post_ms = sum(stage.get(k, 0.0) for k in ("threshold_sort_gather", "nms", "coord_label")) / args.steps
         nms_bytes = nms_algorithmic_bytes(SHAPE[0] * SHAPE[1], n_cand / args.steps, n_inst / args.steps, pairs_per_step, N_RAYS, 2)
         roof_nms = {"name": "nms_labels_2d", "bound": "hbm", "kernel": "threshold/sort/gather + NMS (k_frontier2, k_pairs, k_fast, k_clip) + coord/label painting",
                     "achieved": nms_bytes / (post_ms / 1e3) / 1e9 if post_ms > 0 else 0.0, "peak": peak_bw, "unit": "GB/s",
                     "algorithmic_bytes_per_step": nms_bytes, "ms_per_step": post_ms, "candidates_per_step": n_cand / args.steps,
                     "pairs_per_step": pairs_per_step, "definition": "SURVEY 8d: 4 B/px scan + 2 x 140 B/candidate + 1 B keep + 2 rows per evaluated pair + 4 B/px paint + 1 row per survivor",
-                    "traffic": traffic.get("nms_labels_2d", {}).get("dram_bytes_per_step"), "traffic_source": traffic.get("nms_labels_2d", {}).get("source"),
                     "peak_source": src + " hbm_gbs"}
         roof_nms["frac"] = roof_nms["achieved"] / peak_bw
         out = {
@@ -351,7 +390,7 @@ def main():
                        "candidates_per_image": n_cand / args.steps,
                        "stages_ms": {k: v / args.steps for k, v in stage.items()},
                        "nms_kernels_ms": {k: v["ms"] / args.steps for k, v in prof_nms.items()}},
-            "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
+            "device": gpu_info(local), "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
             "roofline": roof, "roofline_other": {"nms_labels_2d": roof_nms},
         }
     del x_dev
@@ -359,7 +398,7 @@ def main():
     # ------------------------------------------------------------------ configs[2]: 3-D 128x512x512
     if not args.skip_3d:
         try:
-            steps3 = max(2, min(args.steps, 4)); warm3 = 2
+            steps3 = args.steps; warm3 = 2
             cfg3 = bench_data.bench_config_3d(N_RAYS_3D)
             model3 = StarDist3D(cfg3, name=None, basedir=None, weights=bench_data.bench_weights_3d(cfg3))
             vol, _ = bench_data.synthetic_volume(SHAPE_3D, seed=0)
@@ -370,7 +409,10 @@ def main():
             _lib.profile_enable(True)
             l0 = _lib.launch_count()
             barrier()
-            dev_ms3, n_inst3, n_cand3, stage3 = time_device(model3, x3, SHAPE_3D, PROB_THRESH_3D, NMS_THRESH_3D, steps3)
+            dev_ms3, n_inst3, n_cand3, stage3, last3 = time_device(model3, x3, SHAPE_3D, PROB_THRESH_3D, NMS_THRESH_3D, steps3)
+            if args.dump_outputs and rank == 0:
+                dump_outputs(args.dump_outputs, "3d", *last3, label_sample=DUMP_3D_VOXELS)
+            del last3
             launches3 = _lib.launch_count() - l0
             prof_conv3 = _lib.profile_get("conv_tc")
             prof_n3 = {k: _lib.profile_get("nms3d_" + k) for k in ("pretest", "heavy", "heavy_bound", "hulls", "heavy_s4s3s5", "frontier", "paint")}
@@ -399,8 +441,8 @@ def main():
                                       "stages_ms_3d": {k: v / steps3 for k, v in stage3.items()},
                                       "nms3d_kernels_ms": {k: v["ms"] / steps3 for k, v in prof_n3.items() if v["launches"]},
                                       "peak_device_memory_gb_3d": peak_mem})
-                out["roofline_3d"] = {"name": "conv_tc", "bound": "tensor", "kernel": "k_conv_tc4 as the 3x3x3 convolution (tcgen05) + 1x1x1 heads",
-                                      "achieved": ach3, "peak": peak_tf_sust, "unit": "TFLOP/s", "frac": ach3 / peak_tf_sust, "traffic": None,
+                out["roofline_3d"] = {"name": "conv_tc", "bound": "tensor", "kernel": "k_conv_wg as the 3x3x3 convolution (wgmma) + 1x1x1 heads",
+                                      "achieved": ach3, "peak": peak_tf_sust, "unit": "TFLOP/s", "frac": ach3 / peak_tf_sust,
                                       "ms_per_step": c3ms / steps3, "launches_per_step": prof_conv3["launches"] / steps3,
                                       "algorithmic_flop_per_step": prof_conv3["units"] / steps3, "issued_flop_factor": 3, "unet_forward_ms": unet3,
                                       "unet_algorithmic_tflops": fl3 / (unet3 / 1e3) / 1e12 if unet3 > 0 else None,
@@ -408,7 +450,7 @@ def main():
                 out["roofline_other"]["nms_labels_3d"] = {
                     "bound": "hbm", "kernel": "threshold/sort/gather + 3-D NMS (k_pretest, k_heavy, k_frontier) + k_paint3d + relabel",
                     "achieved": b3 / (post3 / 1e3) / 1e9 if post3 > 0 else 0.0, "peak": peak_bw, "unit": "GB/s", "frac": (b3 / (post3 / 1e3) / 1e9 / peak_bw) if post3 > 0 else 0.0,
-                    "algorithmic_bytes_per_step": b3, "ms_per_step": post3, "traffic": traffic.get("nms_labels_3d", {}).get("dram_bytes_per_step"),
+                    "algorithmic_bytes_per_step": b3, "ms_per_step": post3,
                     "definition": "SURVEY 8d: 4 B/voxel scan + 2 x 400 B/candidate + 1 B keep + 4 B/voxel paint + 1 row per survivor (pair rows not counted: no pair counter in 3-D)"}
             del model3, vol
             torch.cuda.empty_cache()
@@ -419,7 +461,7 @@ def main():
             if rank == 0: out["clocks"] = clocks
 
     # ------------------------------------------------------------------ configs[3] / [4]: predict_instances_big sharded over the ranks
-    if not args.skip_big:
+    if args.big:
         def run_big(model_b, img_b, axes, spec, reps):
             kw = dict(axes=axes, block_size=spec["block_size"], min_overlap=spec["min_overlap"], context=spec["context"], show_progress=False)
             res = None
@@ -436,7 +478,7 @@ def main():
         try:
             tile, _ = bench_data.synthetic_image(SHAPE, seed=0)
             big_img = bench_data.TiledImage(tile, tuple(s // t for s, t in zip(BIG_2D["shape"], SHAPE)))
-            times, res = run_big(model, big_img, 'YX', BIG_2D, 2)
+            times, res = run_big(model, big_img, 'YX', BIG_2D, args.steps)
             if rank == 0:
                 t = float(np.median(times))
                 from stardist_b200.big import BlockND
@@ -444,7 +486,7 @@ def main():
                 out["big_2d"] = {"workload": "StarDist2D predict_instances_big, tiled 8192x8192 (configs[3]), block %d / min_overlap %d / context %d -> %d blocks round-robin over %d rank(s)"
                                  % (BIG_2D["block_size"], BIG_2D["min_overlap"], BIG_2D["context"], nblk, world),
                                  "value": res[0] / t, "unit": "instances/s", "seconds": t, "instances": res[0], "scaling": "strong", "n_gpus": world, "blocks": nblk,
-                                 "timed": "wall clock, host tiled image in -> assembled int32 label map + polygons on rank 0's host (max over ranks, median of 2 after 1 warm-up)"}
+                                 "timed": "wall clock, host tiled image in -> assembled int32 label map + polygons on rank 0's host (max over ranks, median of the timed passes after 1 warm-up)", "passes": len(times)}
         except Exception as e:
             if rank == 0: out["big_2d"] = {"error": repr(e)[:400]}
         del model
@@ -455,7 +497,7 @@ def main():
                 model5 = StarDist3D(cfg5, name=None, basedir=None, weights=bench_data.bench_weights_3d(cfg5))
                 cell, _ = bench_data.synthetic_volume(bench_data.CELL_3D, seed=0)
                 big_vol = bench_data.TiledImage(cell, tuple(s // t for s, t in zip(BIG_3D["shape"], cell.shape)))
-                times, res = run_big(model5, big_vol, 'ZYX', BIG_3D, 1)
+                times, res = run_big(model5, big_vol, 'ZYX', BIG_3D, args.steps)
                 if rank == 0:
                     t = float(np.median(times))
                     from stardist_b200.big import BlockND
@@ -463,15 +505,15 @@ def main():
                     out["big_3d"] = {"workload": "StarDist3D predict_instances_big, tiled 512x512x512, rays anisotropy (2,1,1) (configs[4]), block %d / min_overlap %d / context %d -> %d blocks round-robin over %d rank(s)"
                                      % (BIG_3D["block_size"], BIG_3D["min_overlap"], BIG_3D["context"], nblk, world),
                                      "value": res[0] / t, "unit": "instances/s", "seconds": t, "instances": res[0], "scaling": "strong", "n_gpus": world, "blocks": nblk,
-                                     "timed": "wall clock, host tiled volume in -> assembled label volume + polyhedra on rank 0's host (max over ranks, 1 pass after 1 warm-up)"}
+                                     "timed": "wall clock, host tiled volume in -> assembled label volume + polyhedra on rank 0's host (max over ranks, median of the timed passes after 1 warm-up)", "passes": len(times)}
                 del model5
             except Exception as e:
                 if rank == 0: out["big_3d"] = {"error": repr(e)[:400]}
 
     if rank == 0:
-        if not args.no_cpu_baseline and world == 1:
+        if args.cpu_baseline and world == 1:
             try:
-                out["cpu_baseline"] = cpu_baseline_record(reference_numbers(2, 1, budget_s=150.0))
+                out["cpu_baseline"] = cpu_baseline_record(reference_numbers(args.steps, args.warmup, budget_s=150.0))
             except Exception as e:      # the baseline is a report, never a reason to lose the measurement
                 out["cpu_baseline"] = {"error": repr(e)[:300]}
         print(json.dumps(out))

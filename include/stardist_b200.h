@@ -1,4 +1,4 @@
-/* stardist_b200.h -- C ABI of libstardist_b200.so (B200 / sm_100a prediction hot path).
+/* stardist_b200.h -- C ABI of libstardist_b200.so (H100 / sm_90a prediction hot path).
  *
  * Two families of entry points:
  *
@@ -125,7 +125,7 @@ int sdb_polyhedron_to_label(const float* d_dist, const float* d_points, const fl
 /* sphere culling of bounding-box voxels in the 3-D label rendering (1 = default); label maps are identical either way */
 int sdb_label3d_set_cull(int on);
 
-/* k_heavy volume stages (S3 kernel / S4 hull intersection): 0 (default) = per-(k, j) plane scaling as validated on B200,
+/* k_heavy volume stages (S3 kernel / S4 hull intersection): 0 (default) = per-(k, j) plane scaling as validated by the GPU goldens,
  * 1 = planes scaled once per pair + early-out for non-cutting planes (sd3::face_cone_volume_n; bit-identical results on the
  * host build, not yet run on a GPU -- experimental until then). */
 int sdb_nms3d_set_variant(int norm_planes);
@@ -206,9 +206,9 @@ int sdb_heads_2d(const float* d_feat, long long npix, int cfeat, const float* d_
                  const float* d_wd, const float* d_bd, int n_rays, float* d_prob, float* d_dist,
                  sdb_stream_t stream);
 
-/* ---- tcgen05 / TMA / TMEM U-Net path (stardist_b200/csrc/unet_tc.cu) -------------------------
+/* ---- wgmma / TMA U-Net path (stardist_b200/csrc/unet_tc.cu) -------------------------------------
  * Activations are two fp16 planes (hi, lo) per tensor, hi = fp16(v), lo = fp16(v - hi); weights are
- * split the same way into [9][cout][cin] planes by sdb_split_weights.  fp32 accumulation in TMEM. */
+ * split the same way into [9][cout][cin] planes by sdb_split_weights.  fp32 accumulation in registers. */
 int sdb_conv3x3_tc(const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo,
                    int c_src1, int n, int h, int w, const void* w_hi, const void* w_lo, float w_scale, const float* d_bias, int cout,
                    int relu, int up2x, void* out_hi, void* out_lo, sdb_stream_t stream);
@@ -224,13 +224,8 @@ int sdb_conv3x3_heads_tc(const void* src0_hi, const void* src0_lo, int c_src0, c
                          int c_src1, int n, int h, int w, const void* w_hi, const void* w_lo, float w_scale, const float* d_bias,
                          int relu, const float* d_heads_w, const float* d_heads_b, int n_rays, float* d_prob, float* d_dist,
                          sdb_stream_t stream);
-/* profiling aid: time persistent CTAs that only TMA-load (rows x 130 px x box_c channel) boxes of an [1,h,w,c] fp16
- * tensor (no MMA), loads_per_tile boxes per 128-pixel tile; ms_out = milliseconds per pass */
-int sdb_tma_probe(const void* d_act, int h, int w, int c, int box_c, int rows, int loads_per_tile, int reps, float* ms_out, sdb_stream_t stream);
-/* profiling aid: u64 [148][8] wait-cycle counters written by the halo-reuse conv (NULL disables) */
-int sdb_tc_set_debug(void* d_buf);
 /* 3-D U-Net on the tensor cores (model3d.py:360-399): 3x3x3 convolution of ONE volume [d,h,w,c] in split fp16 planes
- * (k_conv_tc4 with the z planes as the tensor map's image axis; weights [27][cout][cin] from sdb_split_weights_3d,
+ * (the z planes as the tensor map's image axis; weights [27][cout][cin] from sdb_split_weights_3d,
  * tap = dz*9 + dy*3 + dx; up2x: 0 none, 2 = nearest 2x2x2 up-sampling written by the epilogue), max-pooling on split
  * planes, and the fp32 -> split conversion behind the CUDA-core stem. */
 int sdb_conv3x3x3_tc(const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo,
@@ -240,13 +235,13 @@ int sdb_split_weights_3d(const float* d_w, int cin, int cout, float w_scale, voi
 int sdb_maxpool3d_split(const void* in_hi, const void* in_lo, int d, int h, int w, int c, int pz, int py, int px,
                         void* out_hi, void* out_lo, sdb_stream_t stream);
 int sdb_split_f32(const float* d_in, long long n, void* out_hi, void* out_lo, sdb_stream_t stream);
-/* kernel variant of sdb_conv3x3_tc: 0 (default) = auto, 1 = one 8x16 tile per CTA, 3 = persistent CTAs with
- * double-buffered TMEM accumulators and merged hi/lo weight tile, 4 = 3 + halo reuse (one box load per
- * 32-channel block, taps as shifted descriptors).  Results are identical up to fp32 summation order. */
+/* kernel variant of sdb_conv3x3_tc: 0 (default) = the measured best, currently the same kernel as 3; 1 = one 8x16 tile per
+ * CTA, 3 = persistent CTAs with 64-channel K blocks where the channel counts allow, 4 = persistent CTAs with 32-channel K blocks
+ * (per-layer timings: tests/tools/conv_layers.py, DESIGN.md 4.1).  Results are identical up to fp32 summation order. */
 int sdb_tc_set_variant(int variant);
-/* 1 (default): the small split-fp16 products (lo*Whi, hi*Wlo) accumulate in their own TMEM columns, the main accumulator
- * takes one truncating tensor-core add per k-step; 0: all products into one accumulator (the round-1 scheme, kept for A/B
- * error measurements: tests/tools/tc_split_error.py).  Applies to every tcgen05 convolution except k_conv_tc4<128>. */
+/* 1 (default): the small split-fp16 products (lo*Whi, hi*Wlo) accumulate in their own registers, the main accumulator
+ * takes one truncating tensor-core add per k-step; 0: all products into one accumulator (kept for A/B error
+ * measurements: tests/tools/tc_split_error.py).  Applies to every tensor-core convolution. */
 int sdb_tc_set_split_acc(int on);
 int sdb_tc_error_check(sdb_stream_t stream);
 /* w_scale: power of two the weights are multiplied by before the split (undone on the accumulator) */

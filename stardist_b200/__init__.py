@@ -1,4 +1,4 @@
-"""stardist_b200 -- B200-native (sm_100a) implementation of StarDist's prediction hot path.
+"""stardist_b200 -- H100-native (sm_90a) implementation of StarDist's prediction hot path.
 
 Public surface mirrors the reference package (`stardist`): StarDist2D / Config2D,
 non_maximum_suppression*, polygons_to_label, dist_to_coord, ... .  All compute runs in

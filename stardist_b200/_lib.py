@@ -64,10 +64,6 @@ def _declare(lib):
     lib.sdb_heads_tc.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, P, P, P]
     lib.sdb_conv3x3_heads_tc.argtypes = [P, P, c_int, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, P, P, c_int, P, P, P]
     lib.sdb_conv3x3_heads_tc.restype = c_int
-    lib.sdb_tma_probe.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_float), P]
-    lib.sdb_tma_probe.restype = c_int
-    lib.sdb_tc_set_debug.argtypes = [P]
-    lib.sdb_tc_set_debug.restype = c_int
     lib.sdb_conv3x3x3_tc.argtypes = [P, P, c_int, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, c_int, P, P, P]
     lib.sdb_conv3x3x3_tc.restype = c_int
     lib.sdb_split_weights_3d.argtypes = [P, c_int, c_int, c_float, P, P, P]
@@ -174,7 +170,7 @@ def launch_count(reset=False):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise StarDistB200Error("stardist_b200 needs a CUDA device (sm_100a); none is visible and there is no CPU fallback")
+        raise StarDistB200Error("stardist_b200 needs a CUDA device (sm_90a); none is visible and there is no CPU fallback")
     return load()
 
 def ptr(t):

@@ -1,11 +1,11 @@
-"""Build libstardist_b200.so (sm_100a) in-tree with nvcc.  Used by __graft_entry__.build()."""
+"""Build libstardist_b200.so (sm_90a) in-tree with nvcc.  Used by __graft_entry__.build()."""
 import os, subprocess, sys, concurrent.futures as cf
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libstardist_b200.so")
 OBJ = os.path.join(CSRC, "_obj")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=default"]
 # translation units; exact=True -> -fmad=false (bit-exact integer/float restatements of the reference)
 UNITS = [

@@ -91,7 +91,7 @@ extern "C" int sdb_label_bbox(const int* d_labels, int ndim, const int* shape, i
   if (!dims_from(ndim, shape, &D, &n) || max_label < 0) { sdb::set_error("label_bbox: bad shape"); return 1; }
   SDB_LAUNCH(k_bbox_init, cdiv(6ll * (max_label + 1), 256), 256, 0, st, d_bbox, max_label + 1);
   SDB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-  if (n > 0) SDB_LAUNCH(k_label_bbox, (int)std::min<long long>(cdiv(n, 256), 148 * 16), 256, 0, st, d_labels, D, n, max_label, d_bbox, d_bad);
+  if (n > 0) SDB_LAUNCH(k_label_bbox, (int)std::min<long long>(cdiv(n, 256), 132 * 16), 256, 0, st, d_labels, D, n, max_label, d_bbox, d_bad);
   return 0;
 }
 
@@ -99,7 +99,7 @@ extern "C" int sdb_label_bbox(const int* d_labels, int ndim, const int* shape, i
 extern "C" int sdb_label_remap(int* d_labels, long long n, const int* d_lut, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n < 0) { sdb::set_error("label_remap: negative size"); return 1; }
-  if (n > 0) SDB_LAUNCH(k_label_remap, (int)std::min<long long>(cdiv(n, 256), 148 * 16), 256, 0, st, d_labels, n, d_lut);
+  if (n > 0) SDB_LAUNCH(k_label_remap, (int)std::min<long long>(cdiv(n, 256), 132 * 16), 256, 0, st, d_labels, n, d_lut);
   return 0;
 }
 
@@ -115,6 +115,6 @@ extern "C" int sdb_label_write(const int* d_tile, int ndim, const int* tile_shap
     o[3 - ndim + i] = origin[i];
     if (origin[i] < 0 || origin[i] + tile_shape[i] > dst_shape[i]) { sdb::set_error("label_write: tile outside the destination"); return 1; }
   }
-  if (n > 0) SDB_LAUNCH(k_label_write, (int)std::min<long long>(cdiv(n, 256), 148 * 16), 256, 0, st, d_tile, T, n, add, d_dst, G, o[0], o[1], o[2]);
+  if (n > 0) SDB_LAUNCH(k_label_write, (int)std::min<long long>(cdiv(n, 256), 132 * 16), 256, 0, st, d_tile, T, n, add, d_dst, G, o[0], o[1], o[2]);
   return 0;
 }

@@ -161,7 +161,7 @@ extern "C" int sdb_threshold_sort(const float* d_prob, int ndim, const int* shap
   SDB_CUDA(b_keys.alloc((size_t)cap_pad * sizeof(u64), st));
   SDB_CUDA(b_count.alloc(sizeof(unsigned int), st));
   SDB_CUDA(cudaMemsetAsync(b_count.p, 0, sizeof(unsigned int), st));
-  const int blocks = (int)std::min<long long>(cdiv(npix, 256), 148 * 16);
+  const int blocks = (int)std::min<long long>(cdiv(npix, 256), 132 * 16);
   SDB_LAUNCH(k_threshold, blocks, 256, 0, st, d_prob, npix, S, prob_thresh, b_keys.as<u64>(), b_count.as<unsigned int>(), (unsigned int)capacity);
   unsigned int n = 0;
   SDB_CUDA(cudaMemcpyAsync(&n, b_count.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(256) k_store_rows(const float* __restrict__ pr
 extern "C" int sdb_count_above(const float* d_prob, long long n, float thresh, int* h_count, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   sdb::DevBuf b; SDB_CUDA(b.alloc(4, st)); SDB_CUDA(cudaMemsetAsync(b.p, 0, 4, st));
-  if (n > 0) SDB_LAUNCH(k_count_above, (int)std::min<long long>(cdiv(n, 1024), 148 * 8), 256, 0, st, d_prob, n, thresh, b.as<unsigned int>());
+  if (n > 0) SDB_LAUNCH(k_count_above, (int)std::min<long long>(cdiv(n, 1024), 132 * 8), 256, 0, st, d_prob, n, thresh, b.as<unsigned int>());
   unsigned int h = 0;
   SDB_CUDA(cudaMemcpyAsync(&h, b.p, 4, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
@@ -244,7 +244,7 @@ extern "C" int sdb_store_rows_above(const float* d_prob, const float* d_dist, lo
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0 || capacity <= 0) return 0;
   sdb::DevBuf b; SDB_CUDA(b.alloc(4, st)); SDB_CUDA(cudaMemsetAsync(b.p, 0, 4, st));
-  SDB_LAUNCH(k_store_rows, (int)std::min<long long>(cdiv(n, 256), 148 * 16), 256, 0, st, d_prob, d_dist, n, n_rays, thresh, flat0, (unsigned int)row0,
+  SDB_LAUNCH(k_store_rows, (int)std::min<long long>(cdiv(n, 256), 132 * 16), 256, 0, st, d_prob, d_dist, n, n_rays, thresh, flat0, (unsigned int)row0,
              (unsigned int)capacity, b.as<unsigned int>(), d_store, d_slot);
   return 0;
 }

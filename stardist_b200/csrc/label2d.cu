@@ -136,7 +136,7 @@ extern "C" int sdb_polygons_to_label_2d(const float* d_coord, const int* d_rank,
   if (n_polys <= 0) return 0;
   SDB_LAUNCH(k_paint, n_polys, 128, 0, st, d_coord, d_rank, n_polys, n_rays, ny, nx, d_out);
   const long long npix = (long long)ny * nx;
-  SDB_LAUNCH(k_rank_to_label, (int)std::min<long long>(cdiv(npix, 256), 148 * 8), 256, 0, st, d_out, npix, d_id_by_rank);
+  SDB_LAUNCH(k_rank_to_label, (int)std::min<long long>(cdiv(npix, 256), 132 * 8), 256, 0, st, d_out, npix, d_id_by_rank);
   return 0;
 }
 

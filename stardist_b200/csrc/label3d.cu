@@ -255,7 +255,7 @@ extern "C" int sdb_polyhedron_to_label(const float* d_dist, const float* d_point
   if (n_rays > MAXR || n_faces > MAXF) { sdb::set_error("polyhedron_to_label: too many rays/faces"); return 1; }
   if (render_mode < 0 || render_mode > 4) { sdb::set_error("polyhedron_to_label: unknown render mode"); return 1; }
   const long long nvox = (long long)nz * ny * nx;
-  const int fb = (int)std::min<long long>(cdiv(nvox, 256), 148 * 16);
+  const int fb = (int)std::min<long long>(cdiv(nvox, 256), 132 * 16);
   if (nvox == 0) return 0;
   // Render mode "full" here is kernel || inside_polyhedron, the reference's is kernel || (hull && inside_polyhedron)
   // (stardist3d_impl.cpp:1475-1477).  inside_polyhedron lies inside the hull -- except for DEGENERATE faces of the ray
@@ -433,7 +433,7 @@ extern "C" int sdb_relabel_sequential(int* d_labels, long long n, int max_label,
   SDB_CUDA(cudaMemsetAsync(d_forward_map, 0, (size_t)(max_label + 3) * sizeof(int), st));
   int* d_count = d_forward_map + max_label + 1;
   int* d_bad = d_forward_map + max_label + 2;
-  const int grid = (int)std::min<long long>(std::max<long long>(cdiv(n >> 2, 256), 1), 148 * 8);
+  const int grid = (int)std::min<long long>(std::max<long long>(cdiv(n >> 2, 256), 1), 132 * 8);
   if (n > 0) SDB_LAUNCH(k_mark_labels, grid, 256, 0, st, d_labels, n, max_label, d_forward_map, d_bad);
   SDB_LAUNCH(k_scan_labels, 1, 1024, 0, st, d_forward_map, max_label, offset, d_count);
   int h[2] = {0, 0};
@@ -471,7 +471,7 @@ extern "C" void _LIB_polyhedron_to_label(const float* dist, const float* points,
   }
   cudaMemcpyAsync(d_verts.p, verts, (size_t)n_rays * 12, cudaMemcpyHostToDevice, st);
   cudaMemcpyAsync(d_faces.p, faces, (size_t)n_faces * 12, cudaMemcpyHostToDevice, st);
-  if (verbose >= 1) printf("+++++++++++++++ polyhedra to label (B200) +++++++++++++++ \nn_polys = %d n_rays = %d n_faces = %d nz,ny,nx = %d %d %d\n", n_polys, n_rays, n_faces, nz, ny, nx);
+  if (verbose >= 1) printf("+++++++++++++++ polyhedra to label (GPU) +++++++++++++++ \nn_polys = %d n_rays = %d n_faces = %d nz,ny,nx = %d %d %d\n", n_polys, n_rays, n_faces, nz, ny, nx);
   if (sdb_polyhedron_to_label(d_dist.as<float>(), d_points.as<float>(), d_verts.as<float>(), d_faces.as<int>(), n_polys, n_rays, n_faces,
                               d_labels.as<int>(), nz, ny, nx, render_mode, use_overlap_label, overlap_label, d_out.as<int>(), (sdb_stream_t)st)) return fail("kernel");
   if (cudaMemcpyAsync(result, d_out.p, (size_t)nvox * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {

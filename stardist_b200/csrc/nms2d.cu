@@ -377,7 +377,7 @@ extern "C" int sdb_nms2d_survivors(const float* d_dist, const float* d_points, i
   SDB_CUDA(cudaMemcpyAsync(b_tab.p, tab.data(), 2 * R * sizeof(float), cudaMemcpyHostToDevice, st));
   const int init_stats[8] = {0, INT32_MAX, INT32_MIN, INT32_MAX, INT32_MIN, 0, 0, 0};
   SDB_CUDA(cudaMemcpyAsync(b_stats.p, init_stats, sizeof(init_stats), cudaMemcpyHostToDevice, st));
-  SDB_LAUNCH(k_precompute_w, std::min(cdiv((long long)n * 32, 256), 148 * 16), 256, 0, st, d_dist, d_points, b_tab.as<float>(), b_tab.as<float>() + R, n, R,
+  SDB_LAUNCH(k_precompute_w, std::min(cdiv((long long)n * 32, 256), 132 * 16), 256, 0, st, d_dist, d_points, b_tab.as<float>(), b_tab.as<float>() + R, n, R,
              b_verts.as<int2>(), b_bbox.as<int4>(), b_radius.as<float>(), b_area.as<float>(),
              filter ? b_suf.as<double>() : (double*)nullptr, b_sarea.as<double>(), b_maxlen.as<float>(), b_stats.as<unsigned int>());
   int h_stats[8];
@@ -440,7 +440,7 @@ extern "C" int sdb_nms2d_survivors(const float* d_dist, const float* d_points, i
   }
 
   if (verbose) {
-    printf("Non Maximum Suppression (2D, B200) ++++ \n");
+    printf("Non Maximum Suppression (2D, GPU) ++++ \n");
     printf("NMS: n_polys    = %d \nNMS: n_rays     = %d  \nNMS: thresh     = %.3f \nNMS: use_bbox   = %d\nNMS: use_kdtree = %d\n", n, R, threshold, use_bbox, use_kdtree);
     printf("NMS: max_dist = %g grid = %d x %d cell = %g\n", max_dist, G.gx, G.gy, G.cell);
   }

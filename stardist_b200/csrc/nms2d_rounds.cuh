@@ -507,8 +507,8 @@ int run_rounds(NmsArrays A, int* d_slow_unused, unsigned int* d_counters, cudaSt
     int* lout = (r & 1) ? b_list0.as<int>() : b_list1.as<int>();
     sdb::ProfSpan spf;
     sdb::profile_begin("nms2d_frontier", st, &spf);
-    if (r == 0) SDB_LAUNCH(k_frontier2, 148 * 8, 256, 0, st, A, r, b_cursor.as<int2>(), b_kept.as<int>(), (const int*)nullptr, (unsigned int)n, (const unsigned int*)nullptr, lout, d_counters);
-    else SDB_LAUNCH(k_frontier2, 148 * 8, 256, 0, st, A, r, b_cursor.as<int2>(), b_kept.as<int>(), (const int*)lin, 0u, (const unsigned int*)(d_counters + 8), lout, d_counters);
+    if (r == 0) SDB_LAUNCH(k_frontier2, 132 * 8, 256, 0, st, A, r, b_cursor.as<int2>(), b_kept.as<int>(), (const int*)nullptr, (unsigned int)n, (const unsigned int*)nullptr, lout, d_counters);
+    else SDB_LAUNCH(k_frontier2, 132 * 8, 256, 0, st, A, r, b_cursor.as<int2>(), b_kept.as<int>(), (const int*)lin, 0u, (const unsigned int*)(d_counters + 8), lout, d_counters);
     sdb::profile_end("nms2d_frontier", st, &spf);
     return 0;
   };
@@ -520,14 +520,14 @@ int run_rounds(NmsArrays A, int* d_slow_unused, unsigned int* d_counters, cudaSt
   auto launch_pair_stage = [&](int r, bool defer_exact = false) -> int {
     sdb::ProfSpan sp;
     sdb::profile_begin("nms2d_pairs", st, &sp);
-    SDB_LAUNCH(k_pairs, 148 * 8, 256, 0, st, A, r, b_kept.as<int>(), b_pairs.as<int2>(), (unsigned int)cap, d_counters);
+    SDB_LAUNCH(k_pairs, 132 * 8, 256, 0, st, A, r, b_kept.as<int>(), b_pairs.as<int2>(), (unsigned int)cap, d_counters);
     sdb::profile_end("nms2d_pairs", st, &sp);
     SDB_LAUNCH(k_check_overflow, 1, 1, 0, st, (unsigned int)cap, d_counters);
     if (filter) {
       sdb::profile_begin("nms2d_fast", st, &sp);
       int* pend = defer_exact ? d_pend : nullptr;
-      if (A.max_abs_coord <= 8191.0) SDB_LAUNCH(k_fast<int32_t>, 148 * 8, 256, 0, st, A, b_pairs.as<int2>(), b_xpairs.as<int2>(), b_verdict.as<signed char>(), filter == 2 ? 1 : 0, d_counters, pend);
-      else SDB_LAUNCH(k_fast<long long>, 148 * 8, 256, 0, st, A, b_pairs.as<int2>(), b_xpairs.as<int2>(), b_verdict.as<signed char>(), filter == 2 ? 1 : 0, d_counters, pend);
+      if (A.max_abs_coord <= 8191.0) SDB_LAUNCH(k_fast<int32_t>, 132 * 8, 256, 0, st, A, b_pairs.as<int2>(), b_xpairs.as<int2>(), b_verdict.as<signed char>(), filter == 2 ? 1 : 0, d_counters, pend);
+      else SDB_LAUNCH(k_fast<long long>, 132 * 8, 256, 0, st, A, b_pairs.as<int2>(), b_xpairs.as<int2>(), b_verdict.as<signed char>(), filter == 2 ? 1 : 0, d_counters, pend);
       sdb::profile_end("nms2d_fast", st, &sp);
       if (defer_exact && filter == 1) return 0;       // the open pairs (counters[9], pend[]) are swept by k_tail
     }
@@ -537,7 +537,7 @@ int run_rounds(NmsArrays A, int* d_slow_unused, unsigned int* d_counters, cudaSt
       const size_t csm = (size_t)CW * sizeof(sdclip::ClipSweep<NV, 1>);
       static bool attr = false;
       if (!attr) { SDB_CUDA(cudaFuncSetAttribute(k_clip<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)csm)); attr = true; }
-      const int cblocks = 148 * (NV <= 32 ? 6 : 4);
+      const int cblocks = 132 * (NV <= 32 ? 6 : 4);
       if (filter == 1) SDB_LAUNCH((k_clip<NV>), cblocks, 32 * CW, csm, st, A, b_xpairs.as<int2>(), d_counters + 9, (const signed char*)nullptr, b_slow.as<int2>(), d_counters);
       else SDB_LAUNCH((k_clip<NV>), cblocks, 32 * CW, csm, st, A, b_pairs.as<int2>(), d_counters + 1, filter == 2 ? b_verdict.as<signed char>() : (const signed char*)nullptr, b_slow.as<int2>(), d_counters);
     }

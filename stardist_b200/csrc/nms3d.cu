@@ -983,7 +983,7 @@ __global__ void k_finish(const int* __restrict__ state, int n, unsigned char* __
 // 0 (default): face_cone_volume as validated on the GPU in round 1; 1: face_cone_volume_n on pre-normalised planes.
 // The two are bit-identical functions (host build, 7 500 fuzzed pairs: tests/test_cpu_oracle.py); the switch exists because
 // variant 1 has not been run on a GPU yet (tests/test_gpu_3d.py runs it under STARDIST_B200_EXPERIMENTAL=1).
-static int g_nms3d_norm_planes = 1;      // face_cone_volume_n (bit-identical on the host build; goldens green on B200, round 2)
+static int g_nms3d_norm_planes = 1;      // face_cone_volume_n (bit-identical on the host build; goldens green on the GPU)
 static int g_nms3d_fan_subdiv = 1;    // refined fan (sdb_nms3d_set_s3_bound(2) = bounds on the coarse fan only)
 static int g_nms3d_s5_bins = 1;       // direction-binned tetrahedra in the S5 rendering (off together with the S3 bound switch)
 static int g_nms3d_warp_bound = 1;    // S3 lower bound by one warp per pair (0: k_heavy stage 1, a CTA per pair)
@@ -1084,7 +1084,7 @@ extern "C" int sdb_nms3d(const float* d_dist, const float* d_points, const float
                       (size_t)n_faces * 12 + 32;      // + face-centroid rays of the refined fan bounds
   SDB_CUDA(cudaFuncSetAttribute(k_heavy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 48 * 1024)));
   if (verbose) {
-    printf("Non Maximum Suppression (3D, B200) ++++ \nNMS: n_polys  = %d \nNMS: n_rays   = %d  \nNMS: n_faces  = %d \nNMS: thresh   = %.3f \nNMS: use_bbox = %d \nNMS: use_kdtree = %d \n",
+    printf("Non Maximum Suppression (3D, GPU) ++++ \nNMS: n_polys  = %d \nNMS: n_rays   = %d  \nNMS: n_faces  = %d \nNMS: thresh   = %.3f \nNMS: use_bbox = %d \nNMS: use_kdtree = %d \n",
            n, n_rays, n_faces, threshold, use_bbox, use_kdtree);
     printf("NMS: calculated anisotropy: %.2f \t %.2f \t %.2f \n", h_aniso[0], h_aniso[1], h_aniso[2]);
   }
@@ -1098,31 +1098,31 @@ extern "C" int sdb_nms3d(const float* d_dist, const float* d_points, const float
     {
       const int* lin = round == 0 ? (const int*)nullptr : ((round & 1) ? b_list1.as<int>() : b_list0.as<int>());
       int* lout = (round & 1) ? b_list0.as<int>() : b_list1.as<int>();
-      SDB_LAUNCH(k_frontier, std::min(cdiv((long long)n * 32, 256), 148 * 8), 256, 0, st, A, round, lin, n, lout, b_kept.as<int>(), b_cursor.as<int2>(), b_counters.as<unsigned int>());
+      SDB_LAUNCH(k_frontier, std::min(cdiv((long long)n * 32, 256), 132 * 8), 256, 0, st, A, round, lin, n, lout, b_kept.as<int>(), b_cursor.as<int2>(), b_counters.as<unsigned int>());
     }
     sdb::profile_end("nms3d_frontier", st, &sp);
     for (;;) {
       sdb::profile_begin("nms3d_pretest", st, &sp);
-      SDB_LAUNCH(k_pretest, 148 * 8, 128, 0, st, A, round, b_kept.as<int>(), b_pairs.as<int2>(), (unsigned int)pair_cap, b_counters.as<unsigned int>());
+      SDB_LAUNCH(k_pretest, 132 * 8, 128, 0, st, A, round, b_kept.as<int>(), b_pairs.as<int2>(), (unsigned int)pair_cap, b_counters.as<unsigned int>());
       sdb::profile_end("nms3d_pretest", st, &sp);
       sdb::profile_begin("nms3d_heavy", st, &sp);
       if (g_nms3d_split) {
         HeavyCtx X{1, b_list4.as<int2>(), b_slot.as<int>(), b_uniq.as<int>(), b_hull.as<Plane>(), b_hulln.as<int>(), hull_cap, FB};
         sdb::ProfSpan s2;
         sdb::profile_begin("nms3d_heavy_bound", st, &s2);
-        if (bound_wpb > 0) SDB_LAUNCH(k_s3_bound_warp, 148 * bound_bps, 256, bound_smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X, bound_wpb);
-        else SDB_LAUNCH(k_heavy, 148 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
+        if (bound_wpb > 0) SDB_LAUNCH(k_s3_bound_warp, 132 * bound_bps, 256, bound_smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X, bound_wpb);
+        else SDB_LAUNCH(k_heavy, 132 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
         sdb::profile_end("nms3d_heavy_bound", st, &s2);
         sdb::profile_begin("nms3d_hulls", st, &s2);
-        SDB_LAUNCH(k_hulls, 148 * 4, 128, hull_smem, st, A, X, b_counters.as<unsigned int>());
+        SDB_LAUNCH(k_hulls, 132 * 4, 128, hull_smem, st, A, X, b_counters.as<unsigned int>());
         sdb::profile_end("nms3d_hulls", st, &s2);
         X.stage = 2;
         sdb::profile_begin("nms3d_heavy_s4s3s5", st, &s2);
-        SDB_LAUNCH(k_heavy, 148 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
+        SDB_LAUNCH(k_heavy, 132 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
         sdb::profile_end("nms3d_heavy_s4s3s5", st, &s2);
       } else {
         HeavyCtx X{0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, FB};
-        SDB_LAUNCH(k_heavy, 148 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
+        SDB_LAUNCH(k_heavy, 132 * 2, 512, smem, st, A, b_pairs.as<int2>(), b_counters.as<unsigned int>(), (unsigned int)pair_cap, X);
       }
       sdb::profile_end("nms3d_heavy", st, &sp);
       if (cudaMemcpyAsync(h_pin, b_counters.p, 64, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {

@@ -137,7 +137,7 @@ SD_HD inline int wind_P_edge(const Edge& e, int32_t qx, int32_t qy) {
 //  * the float32 accumulation of the shoelace sum (area_from_path, stardist2d.cpp:128-138): partial sums
 //    are below n_out·max|coord|·maxlen, n_out additions of relative error 2^-24 each.
 // The geometric part carries a factor 1.25.  tests/tools/polyfast_fuzz.py measures the observed maximum of
-// |area_Clipper − I| / bound over tens of millions of pairs (profiles/r01_polyfast_fuzz.log, DESIGN.md §5).
+// |area_Clipper − I| / bound over tens of millions of pairs (tests/tools/polyfast_fuzz.py, DESIGN.md §5).
 SD_HD inline double clipper_bound(const Accum& acc, double maxlen_sum, double max_abs_coord, int n) {
   const double geom = 1.25 * (0.354 * acc.len + 0.5 * acc.K) + 2.0 * maxlen_sum + 4.0
                       + 4.0e-7 * acc.K * max_abs_coord * maxlen_sum;        // float t, u at the crossings

@@ -153,7 +153,7 @@ extern "C" int sdb_select_ranks(const float* d_x, int ndim, const int* shape, co
   sdb::DevBuf b_state, b_out;
   SDB_CUDA(b_state.alloc(sizeof(SelState), st)); SDB_CUDA(b_out.alloc(MAXQ * sizeof(float), st));
   SDB_CUDA(cudaMemcpyAsync(b_state.p, &hs, sizeof(hs), cudaMemcpyHostToDevice, st));
-  const int grid = (int)std::min<long long>(cdiv(n, 256 * 8), 148 * 8);
+  const int grid = (int)std::min<long long>(cdiv(n, 256 * 8), 132 * 8);
   for (int pass = 0; pass < 4; ++pass) {
     SDB_LAUNCH(k_select_hist, std::max(grid, 1), 256, 0, st, d_x, n, R, pass, n_ranks, b_state.as<SelState>());
     SDB_LAUNCH(k_select_step, 1, 256, 0, st, pass, n_ranks, b_state.as<SelState>(), b_out.as<float>());
@@ -168,7 +168,7 @@ extern "C" int sdb_select_ranks(const float* d_x, int ndim, const int* shape, co
 // in place x = (x - mi) / den (float32, round to nearest) [+ clip to [0,1]] -- csbdeep normalize_mi_ma with den = ma - mi + eps
 extern "C" int sdb_normalize_mi_ma(float* d_x, long long n, float mi, float den, int clip, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  if (n > 0) SDB_LAUNCH(k_normalize, (int)std::min<long long>(cdiv(n, 256 * 4), 148 * 16), 256, 0, st, d_x, n, mi, den, clip);
+  if (n > 0) SDB_LAUNCH(k_normalize, (int)std::min<long long>(cdiv(n, 256 * 4), 132 * 16), 256, 0, st, d_x, n, mi, den, clip);
   return 0;
 }
 
@@ -189,7 +189,7 @@ extern "C" int sdb_zoom_linear(const float* d_in, int ndim, const int* in_shape,
     Z.z[k] = out_shape[a] > 1 ? (double)(in_shape[a] - 1) / (double)(out_shape[a] - 1) : 1.0;
     n_out *= out_shape[a];
   }
-  SDB_LAUNCH(k_zoom_linear, (int)std::min<long long>(cdiv(n_out, 256), 148 * 16), 256, 0, st, d_in, d_out, Z, n_out);
+  SDB_LAUNCH(k_zoom_linear, (int)std::min<long long>(cdiv(n_out, 256), 132 * 16), 256, 0, st, d_in, d_out, Z, n_out);
   return 0;
 }
 
@@ -227,6 +227,6 @@ extern "C" int sdb_pad_reflect_end(const float* d_in, int ndim, const int* in_sh
     P.in[3 - ndim + a] = in_shape[a]; P.out[3 - ndim + a] = out_shape[a]; n_out *= out_shape[a];
     if (out_shape[a] < in_shape[a] || in_shape[a] < 1) { sdb::set_error("pad_reflect_end: bad shapes"); return 1; }
   }
-  SDB_LAUNCH(k_pad_reflect_end, (int)std::min<long long>(cdiv(n_out, 256), 148 * 16), 256, 0, st, d_in, d_out, P, channels, n_out);
+  SDB_LAUNCH(k_pad_reflect_end, (int)std::min<long long>(cdiv(n_out, 256), 132 * 16), 256, 0, st, d_in, d_out, P, channels, n_out);
   return 0;
 }

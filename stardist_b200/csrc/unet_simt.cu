@@ -7,7 +7,7 @@
 // Keras kernels are (kh, kw, Cin, Cout) and the op is a cross-correlation with zero padding.
 //
 // These kernels are the exact-fp32 baseline path (used for the Cin=1 stem, small layers and as
-// the in-repo cross-check of the tcgen05 path in unet_tc.cu).  The decoder's upsample+concat is
+// the in-repo cross-check of the tensor-core path in unet_tc.cu).  The decoder's upsample+concat is
 // folded into the loader's address math: no up-sampled or concatenated tensor is materialised.
 #include <cuda_fp16.h>
 #include <vector>
@@ -351,7 +351,7 @@ extern "C" int sdb_maxpool_nd(const float* d_in, int n, int d, int h, int w, int
   cudaStream_t st = (cudaStream_t)stream;
   if (pz < 1 || py < 1 || px < 1 || d % pz || h % py || w % px || (c & 3)) { sdb::set_error("maxpool_nd: sizes must be divisible by the pool and c % 4 == 0"); return 1; }
   const long long total = (long long)n * (d / pz) * (h / py) * (w / px) * (c / 4);
-  SDB_LAUNCH(k_maxpool_nd, (int)std::min<long long>(cdiv(total, 256), 148 * 16), 256, 0, st, d_in, n, d, h, w, c, pz, py, px, d_out);
+  SDB_LAUNCH(k_maxpool_nd, (int)std::min<long long>(cdiv(total, 256), 132 * 16), 256, 0, st, d_in, n, d, h, w, c, pz, py, px, d_out);
   return 0;
 }
 
@@ -386,13 +386,13 @@ extern "C" int sdb_conv_generic_nd(const float* d_in, int n, int d, int h, int w
   P.od = (d + sz - 1) / sz; P.oh = (h + sy - 1) / sy; P.ow = (w + sx - 1) / sx;
   P.pz = std::max((P.od - 1) * sz + kz - d, 0) / 2; P.py = std::max((P.oh - 1) * sy + ky - h, 0) / 2; P.px = std::max((P.ow - 1) * sx + kx - w, 0) / 2;
   const long long total = (long long)n * P.od * P.oh * P.ow * cout;
-  SDB_LAUNCH(k_conv_generic, (int)std::min<long long>(sdb::cdiv(total, 256), 148 * 64), 256, 0, st, d_in, d_w, d_b, P, d_out);
+  SDB_LAUNCH(k_conv_generic, (int)std::min<long long>(sdb::cdiv(total, 256), 132 * 64), 256, 0, st, d_in, d_w, d_b, P, d_out);
   return 0;
 }
 extern "C" int sdb_add_act(const float* d_a, const float* d_b, long long n, int relu, float* d_out, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) return 0;
-  SDB_LAUNCH(k_add_act, (int)std::min<long long>(sdb::cdiv(n, 256), 148 * 32), 256, 0, st, d_a, d_b, n, relu, d_out);
+  SDB_LAUNCH(k_add_act, (int)std::min<long long>(sdb::cdiv(n, 256), 132 * 32), 256, 0, st, d_a, d_b, n, relu, d_out);
   return 0;
 }
 
@@ -409,6 +409,6 @@ extern "C" int sdb_class_head(const float* d_feat, long long npix, int cfeat, co
 extern "C" int sdb_merge_split(const void* d_hi, const void* d_lo, long long n, float* d_out, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) return 0;
-  SDB_LAUNCH(k_merge_split, (int)std::min<long long>(sdb::cdiv(n, 256), 148 * 32), 256, 0, st, (const __half*)d_hi, (const __half*)d_lo, n, d_out);
+  SDB_LAUNCH(k_merge_split, (int)std::min<long long>(sdb::cdiv(n, 256), 132 * 32), 256, 0, st, (const __half*)d_hi, (const __half*)d_lo, n, d_out);
   return 0;
 }

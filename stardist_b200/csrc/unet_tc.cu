@@ -1,4 +1,4 @@
-// unet_tc.cu -- tcgen05 / TMA / TMEM implicit-GEMM 3x3 convolution for the U-Net backbone (sm_100a).
+// unet_tc.cu -- wgmma / TMA / mbarrier implicit-GEMM 3x3 convolution for the U-Net backbone (sm_90a).
 //
 // Reference op: Keras Conv2D(3x3, padding='same', bias, ReLU) as composed by csbdeep's unet_block
 // (stardist/models/model2d.py:310-349, SURVEY A.1).  Parity target for the float maps is 1e-5
@@ -8,27 +8,23 @@
 //   hi = fp16(v), lo = fp16(v - hi)      (22 significant bits, same 4 bytes/element as fp32)
 // written by the producing kernel's epilogue, and weights are split the same way once per model.
 // A convolution is then 3 fp16 tensor-core passes  hi*Whi + lo*Whi + hi*Wlo  accumulated in fp32
-// in TMEM (each fp16 x fp16 product is exact in fp32; the dropped lo*Wlo term is ~2^-22).
-// Compared with 3xTF32 this doubles the MMA rate (kind::f16) and needs no in-kernel split pass.
+// registers (each fp16 x fp16 product is exact in fp32; the dropped lo*Wlo term is ~2^-22).
+// Compared with 3xTF32 this doubles the MMA rate (fp16 wgmma) and needs no in-kernel split pass.
 //
-// Three kernels share the operand layout (K-major SWIZZLE_128B / SWIZZLE_64B rows written by TMA, one TMEM lane per
-// output pixel, M = 128):
-//   k_conv_tc  : one 8x16-pixel tile per CTA; K loop over (tap, channel block), the A operand of a tap is one 4-D TMA box
-//                {KC channels, 16 x, 8 y, 1 image} at tap-shifted coordinates (out-of-bounds elements are zero-filled by
-//                TMA == the 'same' zero padding).  Kept for Cout = 256.
-//   k_conv_tc3 : the same tiles, persistent CTAs, TMA ring running across tiles, two TMEM accumulator buffers, merged
-//                hi/lo weight tile (two MMAs per k-step instead of three); also the 1x1 heads for n_rays > 32.
-//   k_conv_tc4 : persistent, tile = 2 image rows x 128 pixels, halo loaded once per 32-channel block and the nine taps
-//                addressed by shifted descriptors, weights resident in shared memory where they fit; optionally the
-//                1x1 heads fused into the epilogue (the network's last convolution).  Used for Cin <= 64.
-//   B operand = weights [tap][Cout][Cin] (K-major), 3-D TMA box {KC, N, 1}.
+// One kernel, k_conv_wg<N, KC, FUSE>, does every tensor-core convolution of the network:
+//   tile = 8 x 16 output pixels (M = 128) x N output channels, persistent CTAs sweeping the tiles;
+//   K loop over (tap, KC-channel block): the A operand of a tap is one 4-D TMA box {KC channels, 16 x, 8 y, 1 image}
+//   at tap-shifted coordinates (out-of-bounds elements are zero-filled by TMA == the 'same' zero padding), the B operand
+//   = weights [tap][Cout][Cin] (K-major), 3-D TMA box {KC, N, 1}.  K-major SWIZZLE_128B (KC = 64) / SWIZZLE_64B (KC = 32).
+//   Warp 8 = TMA producer (one lane), warpgroups 0 and 1 = MMA + epilogue for pixel rows [0,64) and [64,128) of the tile.
+//   The producer runs ahead across tile boundaries through a ring of shared-memory stages, so the next tile's loads
+//   overlap the epilogue of the current one.
+//   3x3x3 (n_taps = 27): the tensor map's image axis is the z plane of ONE volume, tap dz reads plane z + dz - 1.
+//   1x1 heads (n_taps = 1): channel 0 -> sigmoid -> prob, channels 1..R -> dist, fp32 outputs.
+//   FUSE: the features convolution (Cout = 128) with the 1x1 heads computed on the fp32 accumulators in the epilogue.
 //   The decoder's Concatenate([UpSampling(x), skip]) is two activation sources on the K axis; the up-sampled source is
-//   materialised by its producer's epilogue (each pixel written 2x2).
-// Warp roles: warp 0 = TMA producer (halos / operand tiles), warp 1 = TMEM alloc + MMA issue (one elected lane of the
-//   converged warp), warps 2.. = epilogue (tcgen05.ld -> bias/ReLU -> hi/lo split -> 16 B global stores, or the fused heads),
-//   k_conv_tc4: last warp = weight TMA.
-// All mbarrier waits are bounded (a hang would cost a GPU-box strike): on timeout an error flag is
-// raised and the kernel drains.
+//   materialised by its producer's epilogue (each pixel written 2x2, or 2x2x2 in 3-D).
+// All mbarrier waits are bounded: on timeout an error flag is raised and the kernel drains.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <vector>
@@ -46,21 +42,20 @@ struct ConvParams {
   int H, W;              // output (== input) spatial size
   int c_src0;            // channels taken from source 0 (0 for a plain convolution)
   int c_total;           // Cin
+  int c_out;             // output channels of the whole layer (row stride of the output planes; N per tile)
   int relu;
-  int up2x;              // write every output pixel to the 2x2 block of a (2H, 2W) tensor
+  int up2x;              // 1: write every output pixel to the 2x2 block of a (2H, 2W) tensor; 2: 2x2x2 block (3-D)
   float acc_scale;       // 2^-k: the weights were multiplied by 2^k before the hi/lo split (keeps w_lo out of the fp16 subnormals)
   const float* bias;
   __half* out_hi; __half* out_lo;
   unsigned int* error_flag;
-  int n_taps;            // 9 (3x3) or 1 (1x1 heads)
+  int n_taps;            // 9 (3x3), 27 (3x3x3) or 1 (1x1 heads)
   int heads_R;           // > 0: heads epilogue -> prob = sigmoid(ch 0), dist = ch 1..R, fp32 outputs
   float* prob; float* dist;
-  // fused features -> heads (k_conv_tc4<128, true>): fp32 head weights [128][36] (columns 0..R-1 = dist, 32 = prob,
-  // zero padded) and biases [36]
+  // fused features -> heads (FUSE): fp32 head weights [128][36] (columns 0..R-1 = dist, 32 = prob, zero padded) and biases [36]
   const float* fuse_w; const float* fuse_b;
-  int split_acc;         // 1: the two small products (lo*Whi, hi*Wlo) accumulate in their own TMEM columns, so the main
-                         // accumulator takes one truncating add per k-step instead of two or three (DESIGN.md 5, network floats)
-  unsigned long long* dbg;      // optional [grid][8] wait-cycle counters of k_conv_tc4 (profiling aid), or nullptr
+  int split_acc;         // 1: the two small products (lo*Whi, hi*Wlo) accumulate in their own registers, so the main
+                         // accumulator takes one truncating add per k-step instead of three (DESIGN.md 5, network floats)
 };
 
 // ---------------------------------------------------------------------------------- PTX helpers
@@ -72,13 +67,16 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
                : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
   return ok != 0;
 }
-// bounded wait: returns false after ~2 s without completion (a hang would cost a GPU-box strike)
+// bounded wait: returns false after ~2 s without completion (a lost arrival then surfaces as an error, not a hang)
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return true;
   unsigned long long t0;
@@ -98,13 +96,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// one elected lane of a fully converged warp (the compiler then issues the uniform-datapath UTCHMMA directly; inside an
-// `if (lane == 0)` region it wraps every MMA in an ELECT / BRA.U.ANY loop, ~60 cycles per instruction)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ float4 lds128(uint32_t saddr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr));
@@ -115,879 +106,366 @@ __device__ __forceinline__ float lds32(uint32_t saddr) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
   return v;
 }
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// K-major shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start addr>>4 [0,14),
-// LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout type [61,64) (2 = SW128, 4 = SW64)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;                               // LBO (unused for swizzled K-major)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;                               // descriptor version (sm_100)
-  d |= (uint64_t)layout_type << 61;
-  return d;
-}
-
-static unsigned long long* g_tc_dbg = nullptr;
-__device__ __forceinline__ bool mbar_wait_t(uint64_t* bar, uint32_t parity, unsigned long long& acc) {
-  const long long t0 = clock64();
-  const bool ok = mbar_wait(bar, parity);
-  acc += (unsigned long long)(clock64() - t0);
-  return ok;
-}
-
-#define SDB_TMEM_LD32(r, taddr)                                                                                        \
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "                                                               \
-               "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                               \
-               "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"               \
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),       \
-                 "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), \
-                 "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), \
-                 "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]) \
-               : "r"(taddr))
-
-// ---------------------------------------------------------------------------------- the kernel
-template <int N, int KC>
-struct TcCfg {
-  static constexpr int ROWB = KC * 2;                       // bytes per operand row
-  static constexpr int A_BYTES = 128 * ROWB;                // one A plane tile
-  static constexpr int B_BYTES = N * ROWB;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  static constexpr int STAGES = (STAGE_BYTES * 4 <= 200 * 1024) ? 4 : ((STAGE_BYTES * 3 <= 200 * 1024) ? 3 : 2);
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-  static constexpr int TMEM_COLS = N <= 32 ? 32 : (N <= 64 ? 64 : (N <= 128 ? 128 : 256));
-  static constexpr int TMEM_ALLOC = 2 * TMEM_COLS;         // second half: correction accumulator (split_acc)
-  static constexpr int NPAD32 = (N + 31) / 32 * 32;
-  static constexpr uint32_t LAYOUT = (ROWB == 128) ? 2u : 4u;
-  static constexpr uint32_t SBO = 8 * ROWB;
-  // instruction descriptor, kind::f16: D=F32 (bit 4), A=B=F16 (0), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-  static constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-};
-
-template <int N, int KC>
-__global__ void __launch_bounds__(192, 1)
-k_conv_tc(const __grid_constant__ CUtensorMap tm_a0_hi, const __grid_constant__ CUtensorMap tm_a0_lo,
-          const __grid_constant__ CUtensorMap tm_a1_hi, const __grid_constant__ CUtensorMap tm_a1_lo,
-          const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, ConvParams P) {
-  using C = TcCfg<N, KC>;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::STAGES;
-  uint64_t* accum_bar = empty_bar + C::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int x0 = blockIdx.x * 16, y0 = blockIdx.y * 8, img = blockIdx.z;
-  const int n_cb = P.c_total / KC;
-  const int n_kb = P.n_taps * n_cb;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)C::TMEM_ALLOC) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      for (int kb = 0; kb < n_kb; ++kb) {
-        const int s = kb % C::STAGES;
-        if (kb >= C::STAGES) {
-          if (!mbar_wait(&empty_bar[s], ((kb / C::STAGES) - 1) & 1)) { atomicExch(P.error_flag, 1u); break; }
-        }
-        const int tap = kb / n_cb, cb = kb % n_cb;
-        const int dy = (P.n_taps == 9) ? tap / 3 - 1 : 0, dx = (P.n_taps == 9) ? tap % 3 - 1 : 0;
-        const int ch = cb * KC;
-        unsigned char* st = smem + s * C::STAGE_BYTES;
-        mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
-        if (ch < P.c_src0) {
-          tma_load_4d(st, &tm_a0_hi, &full_bar[s], ch, x0 + dx, y0 + dy, img);
-          tma_load_4d(st + C::A_BYTES, &tm_a0_lo, &full_bar[s], ch, x0 + dx, y0 + dy, img);
-        } else {
-          tma_load_4d(st, &tm_a1_hi, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, img);
-          tma_load_4d(st + C::A_BYTES, &tm_a1_lo, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, img);
-        }
-        tma_load_3d(st + 2 * C::A_BYTES, &tm_w_hi, &full_bar[s], ch, 0, tap);
-        tma_load_3d(st + 2 * C::A_BYTES + C::B_BYTES, &tm_w_lo, &full_bar[s], ch, 0, tap);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      bool ok = true;
-      for (int kb = 0; kb < n_kb && ok; ++kb) {
-        const int s = kb % C::STAGES;
-        if (!mbar_wait(&full_bar[s], (kb / C::STAGES) & 1)) { atomicExch(P.error_flag, 2u); ok = false; break; }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a_hi = smem_u32(smem + s * C::STAGE_BYTES), a_lo = a_hi + C::A_BYTES;
-        const uint32_t b_hi = a_hi + 2 * C::A_BYTES, b_lo = b_hi + C::B_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < KC / 16; ++ks) {
-          const uint32_t koff = ks * 32;      // 16 fp16 = 32 B along K inside the swizzled row
-          const uint64_t dah = make_desc(a_hi + koff, C::SBO, C::LAYOUT), dal = make_desc(a_lo + koff, C::SBO, C::LAYOUT);
-          const uint64_t dbh = make_desc(b_hi + koff, C::SBO, C::LAYOUT), dbl = make_desc(b_lo + koff, C::SBO, C::LAYOUT);
-          const uint32_t first = (kb | ks) ? 1u : 0u;
-          const uint32_t dcorr = tmem_base + (P.split_acc ? (uint32_t)C::TMEM_COLS : 0u);
-          umma_f16(tmem_base, dah, dbh, C::IDESC, first);
-          umma_f16(dcorr, dal, dbh, C::IDESC, P.split_acc ? first : 1u);
-          umma_f16(dcorr, dah, dbl, C::IDESC, 1u);
-        }
-        tcgen05_commit(&empty_bar[s]);       // frees the smem stage when these MMAs retire
-      }
-      tcgen05_commit(accum_bar);             // accumulator complete (also arrives if we bailed out)
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                  // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;             // pixel row of the tile
-    const int ty = m >> 4, tx = m & 15;
-    const int y = y0 + ty, x = x0 + tx;
-    const bool in_img = (y < P.H) && (x < P.W);
-    const bool ok = mbar_wait(accum_bar, 0);
-    if (!ok) atomicExch(P.error_flag, 3u);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (ok) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < C::NPAD32; c0 += 32) {
-        uint32_t r[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                       "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                       "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                       "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                     : "r"(taddr));
-        if (P.split_acc) {                       // warp-uniform: add the correction accumulator
-          uint32_t r2[32];
-          SDB_TMEM_LD32(r2, taddr + (uint32_t)C::TMEM_COLS);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-        }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (in_img && P.heads_R > 0) {
-          // heads: channel 0 -> sigmoid -> prob, channels 1..R -> dist (fp32)
-          const size_t pix = ((size_t)img * P.H + y) * P.W + x;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int ch = c0 + j;
-            if (ch > P.heads_R) break;
-            const float v = __uint_as_float(r[j]) * P.acc_scale + __ldg(P.bias + ch);
-            if (ch == 0) P.prob[pix] = 1.f / (1.f + expf(-v));
-            else P.dist[pix * P.heads_R + (ch - 1)] = v;
-          }
-        } else if (in_img) {
-          __align__(16) __half hi[32];
-          __align__(16) __half lo[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float v = __uint_as_float(r[j]) * P.acc_scale + __ldg(P.bias + c0 + j);
-            if (P.relu) v = fmaxf(v, 0.f);
-            if (!(fabsf(v) <= 65504.f)) atomicOr(P.error_flag, 0x80000000u);      // fp16 range of the hi plane exceeded (or NaN)
-            const __half h = __float2half_rn(v);
-            hi[j] = h;
-            lo[j] = __float2half_rn(v - __half2float(h));
-          }
-          if (!P.up2x) {
-            const size_t off = (((size_t)img * P.H + y) * P.W + x) * N + c0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-              reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-            }
-          } else {
-            const int H2 = 2 * P.H, W2 = 2 * P.W;
-#pragma unroll
-            for (int rep = 0; rep < 4; ++rep) {
-              const size_t off = (((size_t)img * H2 + (2 * y + (rep >> 1))) * W2 + (2 * x + (rep & 1))) * N + c0;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-                reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-              }
-            }
-          }
-        }
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_ALLOC) : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------- v3: persistent, pipelined across tiles
-// Same tile and operand layout as k_conv_tc, but
-//   * persistent: grid = #SMs, CTA i sweeps tiles i, i+grid, ... ; the TMA ring keeps running across tile
-//     boundaries, so the load latency of a tile hides behind the MMAs of the previous one;
-//   * two TMEM accumulator buffers: the MMA warp fills buffer (t+1)&1 while the epilogue warps drain t&1
-//     (k_conv_tc paid barrier-init + TMEM alloc + pipeline fill + drain per 128 pixels: ~2/3 of its time);
-//   * merged N: W_hi and W_lo tiles sit back to back in shared memory, so  A_hi x [W_hi | W_lo]  is ONE MMA
-//     of width 2N into 2N accumulator columns; the second MMA  A_lo x W_hi  accumulates into the first N.
-//     Two A reads per k-step instead of three (the MMA is shared-memory-read bound for N <= 64), the epilogue
-//     adds the two column groups.  Needs 4N <= 512 TMEM columns: N <= 128.
-template <int N, int KC>
-struct TcCfg3 {
-  static constexpr int ROWB = KC * 2;
-  static constexpr int A_BYTES = 128 * ROWB;
-  static constexpr int B_BYTES = N * ROWB;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-  // N = 48 / 80 / 112 are the padded 1x1 head counts: their epilogue stages the dist rows of a tile in shared memory
-  // (per warp 32 pixels x HSTRIDE floats) and writes them out as contiguous 512-byte warp stores.  HSTRIDE % 32 == 20:
-  // the per-pixel float4 writes of a quarter warp fall into distinct banks.
-  static constexpr bool HEADN = (N == 48 || N == 80 || N == 112);
-  static constexpr int HSTRIDE = N + 4;
-  static constexpr int HSTAGE_BYTES = HEADN ? 4 * 32 * HSTRIDE * 4 : 0;
-  static constexpr int STAGES_RAW = (200 * 1024 - HSTAGE_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + HSTAGE_BYTES;
-  static constexpr int ACC_COLS = (2 * N <= 32) ? 32 : (2 * N <= 64 ? 64 : (2 * N <= 128 ? 128 : 256));   // buffer stride
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static constexpr int NPAD32 = (N + 31) / 32 * 32;
-  static constexpr uint32_t LAYOUT = (ROWB == 128) ? 2u : 4u;
-  static constexpr uint32_t SBO = 8 * ROWB;
-  static constexpr uint32_t IDESC_N = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  static constexpr uint32_t IDESC_2N = (1u << 4) | ((uint32_t)((2 * N) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  static_assert(N % 16 == 0 && 2 * N <= 256, "merged-N variant: N multiple of 16, N <= 128");
-  static_assert((B_BYTES % 1024) == 0 || ROWB == 64, "W_lo tile must start on a swizzle-atom boundary");
-  static_assert(STAGES >= 2, "pipeline needs two stages");
-};
-
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-template <int N, int KC>
-__global__ void __launch_bounds__(192, 1)
-k_conv_tc3(const __grid_constant__ CUtensorMap tm_a0_hi, const __grid_constant__ CUtensorMap tm_a0_lo,
-           const __grid_constant__ CUtensorMap tm_a1_hi, const __grid_constant__ CUtensorMap tm_a1_lo,
-           const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, ConvParams P,
-           int tiles_x, int tiles_y, int n_tiles) {
-  using C = TcCfg3<N, KC>;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + C::STAGES;
-  uint64_t* acc_full = empty_bar + C::STAGES;      // [2]
-  uint64_t* acc_empty = acc_full + 2;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_cb = P.c_total / KC;
-  const int n_kb = P.n_taps * n_cb;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)C::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const int tiles_per_img = tiles_x * tiles_y;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      uint32_t it = 0;
-      bool ok = true;
-      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
-        const int img = tile / tiles_per_img, rem = tile - img * tiles_per_img;
-        const int y0 = (rem / tiles_x) * 8, x0 = (rem % tiles_x) * 16;
-        for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const uint32_t s = it % C::STAGES;
-          if (it >= (uint32_t)C::STAGES) {
-            if (!mbar_wait(&empty_bar[s], ((it / C::STAGES) - 1) & 1)) { atomicExch(P.error_flag, 1u); ok = false; break; }
-          }
-          const int tap = kb / n_cb, cb = kb - tap * n_cb;
-          const int dy = (P.n_taps == 9) ? tap / 3 - 1 : 0, dx = (P.n_taps == 9) ? tap % 3 - 1 : 0;
-          const int ch = cb * KC;
-          unsigned char* st = smem + s * C::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[s], C::STAGE_BYTES);
-          if (ch < P.c_src0) {
-            tma_load_4d(st, &tm_a0_hi, &full_bar[s], ch, x0 + dx, y0 + dy, img);
-            tma_load_4d(st + C::A_BYTES, &tm_a0_lo, &full_bar[s], ch, x0 + dx, y0 + dy, img);
-          } else {
-            tma_load_4d(st, &tm_a1_hi, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, img);
-            tma_load_4d(st + C::A_BYTES, &tm_a1_lo, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, img);
-          }
-          tma_load_3d(st + 2 * C::A_BYTES, &tm_w_hi, &full_bar[s], ch, 0, tap);
-          tma_load_3d(st + 2 * C::A_BYTES + C::B_BYTES, &tm_w_lo, &full_bar[s], ch, 0, tap);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp converged, one elected lane issues) =====================
-    {
-      uint32_t it = 0, t = 0;
-      bool ok = true;
-      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x, ++t) {
-        const uint32_t buf = t & 1;
-        if (t >= 2) {
-          if (!mbar_wait(&acc_empty[buf], ((t >> 1) - 1) & 1)) { atomicExch(P.error_flag, 4u); ok = false; break; }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        const uint32_t d = tmem_base + buf * (uint32_t)C::ACC_COLS;
-        const uint32_t dsplit = P.split_acc ? (uint32_t)N : 0u;
-        for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const uint32_t s = it % C::STAGES;
-          if (!mbar_wait(&full_bar[s], (it / C::STAGES) & 1)) { atomicExch(P.error_flag, 2u); ok = false; break; }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a_hi = smem_u32(smem + s * C::STAGE_BYTES), a_lo = a_hi + C::A_BYTES;
-          const uint32_t b_hi = a_hi + 2 * C::A_BYTES;          // W_hi rows, W_lo rows directly behind
-          // descriptors once per stage, then +2 per 16-element k-step (address field = addr >> 4)
-          const uint64_t dah0 = make_desc(a_hi, C::SBO, C::LAYOUT), dal0 = make_desc(a_lo, C::SBO, C::LAYOUT);
-          const uint64_t dbh0 = make_desc(b_hi, C::SBO, C::LAYOUT);
-#pragma unroll
-          for (int ks = 0; ks < KC / 16; ++ks) {
-            if (elect_one()) umma_f16(d, dah0 + 2u * ks, dbh0 + 2u * ks, C::IDESC_2N, (kb | ks) ? 1u : 0u);      // cols [0,N): hi*Whi, [N,2N): hi*Wlo
-            if (elect_one()) umma_f16(d + dsplit, dal0 + 2u * ks, dbh0 + 2u * ks, C::IDESC_N, 1u);                // lo*Whi -> cols [0,N), or [N,2N) with split_acc
-          }
-          if (elect_one()) tcgen05_commit(&empty_bar[s]);
-        }
-        if (elect_one()) tcgen05_commit(&acc_full[buf]);        // (arrives even after a bail-out so the epilogue does not wait forever)
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const int ty = m >> 4, tx = m & 15;
-    uint32_t t = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t buf = t & 1;
-      const int img = tile / tiles_per_img, rem = tile - img * tiles_per_img;
-      const int y = (rem / tiles_x) * 8 + ty, x = (rem % tiles_x) * 16 + tx;
-      const bool in_img = (y < P.H) && (x < P.W);
-      if (!mbar_wait(&acc_full[buf], (t >> 1) & 1)) { atomicExch(P.error_flag, 3u); break; }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)C::ACC_COLS;
-      if (C::HEADN && P.heads_R > 0 && (P.heads_R & 3) == 0) {
-        // ---- 1x1 heads, coalesced: channel 0 -> sigmoid -> prob; channels 1..R -> dist rows staged per warp in shared
-        // memory (thread = pixel writes float4 pieces of ITS row), then the warp streams the two 16-pixel image rows it
-        // owns -- 16 * R contiguous floats each in HBM -- as 512-byte stores.  (One scalar store per (pixel, ray) was
-        // 32 four-byte pieces 4*R bytes apart per instruction: 1.1 TB/s on the 3-D heads, profiles/r01x.)
-        const int R = P.heads_R, R4 = R >> 2;
-        float* stg = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 256) + (size_t)q * 32 * C::HSTRIDE;
-        float* myrow = stg + lane * C::HSTRIDE;
-        float c29 = 0.f, c30 = 0.f, c31 = 0.f;
-#pragma unroll 1
-        for (int c0 = 0; c0 < C::NPAD32; c0 += 32) {
-          uint32_t r[32], r2[32];
-          SDB_TMEM_LD32(r, tbase + (uint32_t)c0);
-          SDB_TMEM_LD32(r2, tbase + (uint32_t)(N + c0));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (c0 + 32 >= C::NPAD32) {
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-          }
-          float v[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int ch = c0 + j;
-            v[j] = (ch <= R) ? (__uint_as_float(r[j]) + __uint_as_float(r2[j])) * P.acc_scale + __ldg(P.bias + ch) : 0.f;
-          }
-          if (c0 == 0) {
-            if (in_img) P.prob[((size_t)img * P.H + y) * P.W + x] = 1.f / (1.f + expf(-v[0]));
-          } else if (c0 - 1 < R) {                 // dist c0-4 .. c0-1: three carried values + channel c0
-            *reinterpret_cast<float4*>(myrow + c0 - 4) = make_float4(c29, c30, c31, v[0]);
-          }
-#pragma unroll
-          for (int g = 0; g < 7; ++g)               // dist c0+4g .. c0+4g+3 = channels c0+4g+1 .. c0+4g+4
-            if (c0 + 4 * g + 3 < R) *reinterpret_cast<float4*>(myrow + c0 + 4 * g) = make_float4(v[4 * g + 1], v[4 * g + 2], v[4 * g + 3], v[4 * g + 4]);
-          c29 = v[29]; c30 = v[30]; c31 = v[31];
-        }
-        __syncwarp();
-        const int ty0 = (rem / tiles_x) * 8 + 2 * q, x0 = (rem % tiles_x) * 16;
-        const int nx = min(16, P.W - x0);
-#pragma unroll 1
-        for (int rr = 0; rr < 2; ++rr) {
-          const int yy = ty0 + rr;
-          if (yy >= P.H) break;
-          float4* g = reinterpret_cast<float4*>(P.dist + (((size_t)img * P.H + yy) * P.W + x0) * R);
-          const float* srow = stg + rr * 16 * C::HSTRIDE;
-          const int n4 = nx * R4;
-          for (int f = lane; f < n4; f += 32) {
-            const int px = f / R4, k4 = f - px * R4;
-            g[f] = *reinterpret_cast<const float4*>(srow + px * C::HSTRIDE + 4 * k4);
-          }
-        }
-        __syncwarp();                              // the staging rows are rewritten by the next tile
-        continue;
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < C::NPAD32; c0 += 32) {
-        uint32_t r[32], r2[32];
-        SDB_TMEM_LD32(r, tbase + (uint32_t)c0);
-        SDB_TMEM_LD32(r2, tbase + (uint32_t)(N + c0));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (c0 + 32 >= C::NPAD32) {
-          // all TMEM reads of this tile are done: hand the buffer back to the MMA warp
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[buf]);
-        }
-        if (in_img && P.heads_R > 0) {
-          // heads: channel 0 -> sigmoid -> prob, channels 1..R -> dist (fp32)
-          const size_t pix = ((size_t)img * P.H + y) * P.W + x;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int ch = c0 + j;
-            if (ch > P.heads_R) break;
-            const float v = (__uint_as_float(r[j]) + __uint_as_float(r2[j])) * P.acc_scale + __ldg(P.bias + ch);
-            if (ch == 0) P.prob[pix] = 1.f / (1.f + expf(-v));
-            else P.dist[pix * P.heads_R + (ch - 1)] = v;
-          }
-          continue;
-        }
-        if (in_img) {
-          __align__(16) __half hi[32];
-          __align__(16) __half lo[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float v = (__uint_as_float(r[j]) + __uint_as_float(r2[j])) * P.acc_scale + __ldg(P.bias + c0 + j);
-            if (P.relu) v = fmaxf(v, 0.f);
-            if (!(fabsf(v) <= 65504.f)) atomicOr(P.error_flag, 0x80000000u);      // fp16 range of the hi plane exceeded (or NaN)
-            const __half h = __float2half_rn(v);
-            hi[j] = h;
-            lo[j] = __float2half_rn(v - __half2float(h));
-          }
-          if (!P.up2x) {
-            const size_t off = (((size_t)img * P.H + y) * P.W + x) * N + c0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-              reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-            }
-          } else {
-            const int H2 = 2 * P.H, W2 = 2 * P.W;
-#pragma unroll
-            for (int rep = 0; rep < 4; ++rep) {
-              const size_t off = (((size_t)img * H2 + (2 * y + (rep >> 1))) * W2 + (2 * x + (rep & 1))) * N + c0;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-                reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-              }
-            }
-          }
-        }
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS) : "memory");
-  }
-}
-
-// K-major SWIZZLE_64B descriptor (rows of 64 bytes, 8-row atoms of 512 B).  Tap-shifted start addresses are multiples
-// of 64 B, not of the atom: the swizzle is a function of the absolute shared-memory address bits, which TMA (writer) and
-// the MMA (reader) both apply, so no base-offset correction is needed (validated against fp64 convolutions).
-__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr, int /*unused*/) {
+// K-major swizzled shared-memory matrix descriptor of wgmma: start addr>>4 [0,14), LBO>>4 [16,30) (unused for swizzled
+// K-major), SBO>>4 [32,46) = stride of 8-row groups, swizzle mode [62,64) (1 = 128B, 2 = 64B).  Operand tiles start on
+// 1024-byte boundaries, so the base-offset field stays 0; a k-step of 16 fp16 (32 B) inside the swizzled row is +2.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t swizzle) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512 >> 4) << 32;                      // SBO: 8 rows x 64 B
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)4 << 61;                               // SWIZZLE_64B
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)swizzle << 62;
   return d;
 }
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int K> __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(K) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R> __device__ __forceinline__ void wg_fence_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// ---------------------------------------------------------------------------------- v4: persistent + halo reuse
-// Data movement: the (S+2) x 130 pixel halo of a 32-channel block is loaded ONCE (one 4-D TMA box per plane) and the
-// nine taps are shifted UMMA descriptors into it (rows of a strip are contiguous 64-byte rows of the halo, so tap
-// (dy,dx) is just a different start address); schedule as in k_conv_tc3 (persistent CTAs, TMA ring running across
-// tiles, two TMEM accumulator buffers, merged hi/lo weight tile where the columns allow it).  For the
-// high-resolution, few-channel layers (Cin <= 64) the per-tap A re-fetch of k_conv_tc/k_conv_tc3 made them
-// L2->SMEM bound (180 KB per 128 pixels at Cin = 32); here it is ~50 KB.
-//   tile = S = 2 image rows x 128 pixels; accumulators: S x (MERGE ? 2N : N) TMEM columns per buffer.
-template <int N>
-struct TcCfg4 {
-  static constexpr int S = 2, KC = 32, ROWB = 64;
-  static constexpr bool MERGE = (N <= 64);
-  static constexpr int HROWS = (S + 2) * 130;
-  static constexpr int A_PLANE = ((HROWS * ROWB + 1023) / 1024) * 1024;
-  static constexpr int A_STAGE = 2 * A_PLANE;
-  static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGE = 2 * N * ROWB;
-  // weight ring depth when the layer's weights do not stay resident (see WRES): the slot of a tap is recycled only
-  // after its MMAs retired (tcgen05.commit) plus a TMA round trip, ~2 us -- a shallow ring starves the tensor pipe
-  // Ring slots are handed over in groups of BG consecutive taps (one mbarrier wait + one tcgen05.commit per group): with a
-  // wait and a commit per tap the issuing thread spent ~220 of ~650 cycles per tap on them (N = 32, tests/tools/tc4_waits_3d.py).
-  static constexpr int BG = (N >= 128) ? 1 : 3;
-  static constexpr int B_STAGES = (N >= 128) ? 4 : (N == 64 ? 9 : 21);    // N = 32: only the 3-D layers (27 taps x 4 KB > W_RESIDENT_MAX) use the ring
-  static constexpr int B_GROUPS = B_STAGES / BG;
-  static_assert(B_STAGES % BG == 0 && 9 % BG == 0 && B_GROUPS >= 2, "weight ring groups");
-  static constexpr int W_RESIDENT_MAX = 88 * 1024;         // 9 * n_cb * B_STAGE up to this size stays in shared memory
-  static constexpr int SMEM_FIXED = A_STAGES * A_STAGE + 1024 /*align*/ + 512 /*barriers*/;
-  static constexpr int STRIP_COLS = MERGE ? 2 * N : N;
-  static constexpr int ACC_COLS = S * STRIP_COLS;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;           // 256 (N=32) / 512 (N=64, N=128)
-  static constexpr uint32_t IDESC_N = (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  static constexpr uint32_t IDESC_2N = (1u << 4) | ((uint32_t)((2 * N) >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  static_assert(N == 32 || N == 64 || N == 128, "N in {32, 64, 128}");
-  static_assert(TMEM_COLS <= 512, "accumulators exceed TMEM");
-  static_assert(SMEM_FIXED + B_STAGES * B_STAGE <= 227 * 1024, "shared memory");
+// wgmma.m64nNk16.f32.f16.f16, A and B from shared memory (K-major), D += A x B^T (acc = 0: D = A x B^T).
+// Accumulator fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[j] holds row w*16 + l/4 + 8*((j/2)&1),
+// column (j/4)*8 + (l%4)*2 + (j&1).
+template <int N> struct Wg;
+template <> struct Wg<32> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<48> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %26, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<64> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<80> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                 "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<112> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %58, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                 "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<128> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                 "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
+                 "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+               : "l"(a), "l"(b), "r"(acc));
+  }
+};
+template <> struct Wg<144> {
+  __device__ __forceinline__ static void mma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %74, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n144k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1, 0, 0;\n}\n"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                 "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                 "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                 "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                 "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
+                 "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+               : "l"(a), "l"(b), "r"(acc));
+  }
 };
 
-// WRES: all 9 * n_cb weight tiles of the layer are loaded ONCE per (persistent) CTA and stay in shared memory.
-template <int N, bool FUSE, bool WRES>
-__global__ void __launch_bounds__(FUSE ? 352 : 224, 1)
-k_conv_tc4(const __grid_constant__ CUtensorMap tm_a0_hi, const __grid_constant__ CUtensorMap tm_a0_lo,
-           const __grid_constant__ CUtensorMap tm_a1_hi, const __grid_constant__ CUtensorMap tm_a1_lo,
-           const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, ConvParams P,
-           int tiles_x, int tiles_y, int n_tiles, int n_b_slots, int n_dz) {
-  using C = TcCfg4<N>;
-  constexpr int S = C::S;
-  constexpr int RG = C::B_GROUPS;                // weight ring depth in groups of C::BG taps
-  constexpr int W_WARP = FUSE ? 10 : 6;          // warps: 0 halo TMA, 1 MMA, 2.. epilogue (4 or 8), last: weight TMA
+// ---------------------------------------------------------------------------------- the kernel
+template <int N, int KC, bool FUSE>
+struct WgCfg {
+  static constexpr int ROWB = KC * 2;                       // bytes per operand row
+  static constexpr int A_BYTES = 128 * ROWB;                // one A plane tile (a multiple of 1024)
+  static constexpr int B_BYTES = N * ROWB;
+  static constexpr int B_SLOT = (B_BYTES + 1023) / 1024 * 1024;
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_SLOT;
+  static constexpr int TX_BYTES = 2 * A_BYTES + 2 * B_BYTES;
+  static constexpr int FUSE_BYTES = FUSE ? (36 + N + N * 36) * 4 : 0;   // head biases, feature biases, head weights
+  static constexpr int STAGES_RAW = (216 * 1024 - FUSE_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/ + FUSE_BYTES;
+  static constexpr uint32_t SWZ = (ROWB == 128) ? 1u : 2u;
+  static constexpr uint32_t SBO = 8 * ROWB;
+  static constexpr int NREG = N / 2;                        // accumulator registers per thread (m64nN over 128 threads)
+  static_assert(N % 16 == 0 && N <= 256, "wgmma N");
+  static_assert(STAGES >= 2, "pipeline needs two stages");
+  static_assert(SMEM <= 227 * 1024, "shared memory");
+  static_assert(!FUSE || N == 128, "fused heads follow the 128-channel features convolution");
+};
+
+constexpr int kConsumerThreads = 256;                       // two warpgroups
+constexpr int kThreads = kConsumerThreads + 128;            // + the producer warpgroup (one TMA lane)
+// register split (setmaxnreg): the producer warpgroup needs few, the accumulators (2 x N/2 floats) need many;
+// 128 * 40 + 256 * 232 <= 64K registers
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+
+template <int N, int KC, bool FUSE>
+__global__ void __launch_bounds__(kThreads, 1)
+k_conv_wg(const __grid_constant__ CUtensorMap tm_a0_hi, const __grid_constant__ CUtensorMap tm_a0_lo,
+          const __grid_constant__ CUtensorMap tm_a1_hi, const __grid_constant__ CUtensorMap tm_a1_lo,
+          const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, ConvParams P,
+          int tiles_x, int tiles_y, int n_nb, int n_tiles) {
+  using C = WgCfg<N, KC, FUSE>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* smA = smem;
-  unsigned char* smB = smem + C::A_STAGES * C::A_STAGE;
-  // n_b_slots = B_STAGES (ring) or 9 * n_cb (resident weights)
-  uint64_t* a_full = reinterpret_cast<uint64_t*>(smB + (size_t)n_b_slots * C::B_STAGE);
-  uint64_t* a_empty = a_full + C::A_STAGES;
-  uint64_t* b_full = a_empty + C::A_STAGES;        // ring: [B_STAGES]; resident: [0] = "all weights landed"
-  uint64_t* b_empty = b_full + C::B_STAGES;
-  uint64_t* acc_full = b_empty + C::B_STAGES;      // [2]
-  uint64_t* acc_empty = acc_full + 2;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* sHW = reinterpret_cast<float*>(smB + (size_t)n_b_slots * C::B_STAGE + 512);   // FUSE: biases + exchange area
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + C::STAGES;
+  float* sHW = reinterpret_cast<float*>(smem + C::STAGES * C::STAGE_BYTES + 256);   // FUSE only
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_cb = P.c_total / C::KC;
+  const int n_cb = P.c_total / KC;
+  const int n_kb = P.n_taps * n_cb;
 
-  if (FUSE) {      // head biases [36], feature biases [N], head weights [N][36]
+  if (FUSE) {
     for (int e = threadIdx.x; e < 36; e += blockDim.x) sHW[e] = P.fuse_b[e];
     for (int e = threadIdx.x; e < N; e += blockDim.x) sHW[36 + e] = P.bias[e];
     for (int e = threadIdx.x; e < N * 36; e += blockDim.x) sHW[36 + N + e] = P.fuse_w[e];
   }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < C::A_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < C::B_STAGES; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], FUSE ? 8 : 4); }
+    // empty: one arrival per consumer warp once its MMAs on the stage have retired
+    for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsumerThreads / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)C::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  const int tiles_per_img = tiles_x * tiles_y;
 
-  if (warp == 0) {
+  if (warp >= kConsumerThreads / 32) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      uint32_t ai = 0;
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp == kConsumerThreads / 32 && lane == 0) {
+      uint32_t it = 0;
       bool ok = true;
-      unsigned long long w_prod = 0;
-      // halos run ahead by A_STAGES work items (tile, channel block), independent of the weight ring
-      // 3-D (n_dz == 3): the "image" coordinate of the tensor map is the z plane of ONE volume; plane z of the output
-      // accumulates the 3x3 taps of planes z-1, z, z+1 (planes outside the volume are out of bounds = zero filled)
-      auto load_halo = [&](int tile, int cb, int dz, uint32_t a_idx) -> bool {
-        const int img = tile / tiles_per_img, rem = tile - img * tiles_per_img;
-        const int y0 = (rem / tiles_x) * S, x0 = (rem % tiles_x) * 128;
-        const int plane = img + dz - (n_dz == 3 ? 1 : 0);
-        const uint32_t sa = a_idx % C::A_STAGES;
-        if (a_idx >= (uint32_t)C::A_STAGES && !mbar_wait_t(&a_empty[sa], ((a_idx / C::A_STAGES) - 1) & 1, w_prod)) { atomicExch(P.error_flag, 11u); return false; }
-        const int ch = cb * C::KC;
-        unsigned char* sta = smA + sa * C::A_STAGE;
-        mbar_expect_tx(&a_full[sa], 2 * C::HROWS * C::ROWB);
-        if (ch < P.c_src0) {
-          tma_load_4d(sta, &tm_a0_hi, &a_full[sa], ch, x0 - 1, y0 - 1, plane);
-          tma_load_4d(sta + C::A_PLANE, &tm_a0_lo, &a_full[sa], ch, x0 - 1, y0 - 1, plane);
-        } else {
-          tma_load_4d(sta, &tm_a1_hi, &a_full[sa], ch - P.c_src0, x0 - 1, y0 - 1, plane);
-          tma_load_4d(sta + C::A_PLANE, &tm_a1_lo, &a_full[sa], ch - P.c_src0, x0 - 1, y0 - 1, plane);
-        }
-        return true;
-      };
-      int tile = blockIdx.x, cb = 0, dz = 0;
-      while (ok && tile < n_tiles) {
-        ok = load_halo(tile, cb, dz, ai);
-        ++ai;
-        if (++dz == n_dz) { dz = 0; if (++cb == n_cb) { cb = 0; tile += (int)gridDim.x; } }
-      }
-      if (P.dbg) P.dbg[blockIdx.x * 8 + 6] = w_prod;
-    }
-  } else if (warp == W_WARP) {
-    // ===================== TMA producer: weights (own warp: the halo requests must not queue behind ring waits) ==========
-    if (lane == 0) {
-      uint32_t bi = 0;
-      bool ok = true;
-      if (WRES) {
-        mbar_expect_tx(&b_full[0], (uint32_t)(9 * n_dz * n_cb) * C::B_STAGE);
-        for (int cb = 0; cb < n_cb; ++cb)
-          for (int tap = 0; tap < 9 * n_dz; ++tap) {
-            unsigned char* stb = smB + (size_t)(cb * 9 * n_dz + tap) * C::B_STAGE;
-            tma_load_3d(stb, &tm_w_hi, &b_full[0], cb * C::KC, 0, tap);
-            tma_load_3d(stb + N * C::ROWB, &tm_w_lo, &b_full[0], cb * C::KC, 0, tap);
+      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
+        const int nb = tile % n_nb, r = tile / n_nb;
+        const int bx = r % tiles_x, by = (r / tiles_x) % tiles_y, img = r / (tiles_x * tiles_y);
+        const int x0 = bx * 16, y0 = by * 8;
+        for (int kb = 0; kb < n_kb; ++kb, ++it) {
+          const uint32_t s = it % C::STAGES;
+          if (it >= (uint32_t)C::STAGES && !mbar_wait(&empty_bar[s], ((it / C::STAGES) - 1) & 1)) {
+            atomicExch(P.error_flag, 1u); ok = false; break;
           }
+          const int tap = kb / n_cb, cb = kb - tap * n_cb;
+          const int t9 = tap % 9;
+          const int dy = (P.n_taps == 1) ? 0 : t9 / 3 - 1, dx = (P.n_taps == 1) ? 0 : t9 % 3 - 1;
+          const int plane = (P.n_taps == 27) ? img + tap / 9 - 1 : img;
+          const int ch = cb * KC;
+          unsigned char* st = smem + s * C::STAGE_BYTES;
+          mbar_expect_tx(&full_bar[s], C::TX_BYTES);
+          if (ch < P.c_src0) {
+            tma_load_4d(st, &tm_a0_hi, &full_bar[s], ch, x0 + dx, y0 + dy, plane);
+            tma_load_4d(st + C::A_BYTES, &tm_a0_lo, &full_bar[s], ch, x0 + dx, y0 + dy, plane);
+          } else {
+            tma_load_4d(st, &tm_a1_hi, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, plane);
+            tma_load_4d(st + C::A_BYTES, &tm_a1_lo, &full_bar[s], ch - P.c_src0, x0 + dx, y0 + dy, plane);
+          }
+          tma_load_3d(st + 2 * C::A_BYTES, &tm_w_hi, &full_bar[s], ch, nb * N, tap);
+          tma_load_3d(st + 2 * C::A_BYTES + C::B_SLOT, &tm_w_lo, &full_bar[s], ch, nb * N, tap);
+        }
+      }
+    }
+    return;
+  }
+
+  // ===================== MMA + epilogue (warpgroup wg: pixel rows [64 wg, 64 wg + 64) of the tile) =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
+  const int wg = threadIdx.x >> 7, w = warp & 3;
+  float acc[C::NREG], cor[C::NREG];
+#pragma unroll
+  for (int j = 0; j < C::NREG; ++j) cor[j] = 0.f;
+  uint32_t it = 0;
+  bool ok = true;
+  for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x) {
+    const int nb = tile % n_nb, r = tile / n_nb;
+    const int bx = r % tiles_x, by = (r / tiles_x) % tiles_y, img = r / (tiles_x * tiles_y);
+    wg_fence_regs<C::NREG>(acc); wg_fence_regs<C::NREG>(cor);
+    for (int kb = 0; kb < n_kb; ++kb, ++it) {
+      const uint32_t s = it % C::STAGES;
+      ok = __all_sync(0xffffffffu, mbar_wait(&full_bar[s], (it / C::STAGES) & 1));
+      if (!ok) { atomicExch(P.error_flag, 2u); break; }
+      const uint32_t a_hi = smem_u32(smem + s * C::STAGE_BYTES) + (uint32_t)(wg * 64 * C::ROWB), a_lo = a_hi + C::A_BYTES;
+      const uint32_t b_hi = smem_u32(smem + s * C::STAGE_BYTES) + 2 * C::A_BYTES, b_lo = b_hi + C::B_SLOT;
+      const uint64_t dah = make_desc(a_hi, C::SBO, C::SWZ), dal = make_desc(a_lo, C::SBO, C::SWZ);
+      const uint64_t dbh = make_desc(b_hi, C::SBO, C::SWZ), dbl = make_desc(b_lo, C::SBO, C::SWZ);
+      wg_fence();
+      if (P.split_acc) {
+#pragma unroll
+        for (int ks = 0; ks < KC / 16; ++ks) {
+          const uint32_t first = (kb | ks) ? 1u : 0u;
+          Wg<N>::mma(acc, dah + 2u * ks, dbh + 2u * ks, first);
+          Wg<N>::mma(cor, dal + 2u * ks, dbh + 2u * ks, first);
+          Wg<N>::mma(cor, dah + 2u * ks, dbl + 2u * ks, 1u);
+        }
       } else {
-        for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x)
-          for (int cb = 0; cb < n_cb && ok; ++cb) {
-            const int ch = cb * C::KC;
-            for (int tap = 0; tap < 9 * n_dz; tap += C::BG, ++bi) {       // tap index = dz * 9 + (dy * 3 + dx); bi counts groups
-              const uint32_t gs = bi % RG;
-              if (bi >= (uint32_t)RG && !mbar_wait(&b_empty[gs], ((bi / RG) - 1) & 1)) { atomicExch(P.error_flag, 12u); ok = false; break; }
-              mbar_expect_tx(&b_full[gs], (uint32_t)C::BG * C::B_STAGE);
 #pragma unroll
-              for (int k = 0; k < C::BG; ++k) {
-                unsigned char* stb = smB + (size_t)(gs * C::BG + k) * C::B_STAGE;
-                tma_load_3d(stb, &tm_w_hi, &b_full[gs], ch, 0, tap + k);
-                tma_load_3d(stb + N * C::ROWB, &tm_w_lo, &b_full[gs], ch, 0, tap + k);
-              }
-            }
-          }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (whole warp converged, one elected lane issues) =====================
-    {
-      uint32_t ai = 0, bi = 0, t = 0;
-      bool ok = true;
-      unsigned long long w_m0 = 0, w_m1 = 0, w_m2 = 0;
-      const long long t_m = clock64();
-      if (WRES && !mbar_wait(&b_full[0], 0)) { atomicExch(P.error_flag, 17u); ok = false; }
-      for (int tile = blockIdx.x; tile < n_tiles && ok; tile += gridDim.x, ++t) {
-        const uint32_t buf = t & 1;
-        if (t >= 2) {
-          if (!mbar_wait_t(&acc_empty[buf], ((t >> 1) - 1) & 1, w_m0)) { atomicExch(P.error_flag, 16u); ok = false; break; }
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        for (int ks = 0; ks < KC / 16; ++ks) {
+          Wg<N>::mma(acc, dah + 2u * ks, dbh + 2u * ks, (kb | ks) ? 1u : 0u);
+          Wg<N>::mma(acc, dal + 2u * ks, dbh + 2u * ks, 1u);
+          Wg<N>::mma(acc, dah + 2u * ks, dbl + 2u * ks, 1u);
         }
-        const uint32_t d0 = tmem_base + buf * (uint32_t)C::ACC_COLS;
-        const uint32_t dsplit = (C::MERGE && P.split_acc) ? (uint32_t)N : 0u;
-        for (int cbz = 0; cbz < n_cb * n_dz && ok; ++cbz, ++ai) {
-          const int cb = cbz / n_dz, dz = cbz - cb * n_dz;
-          const uint32_t sa = ai % C::A_STAGES;
-          if (!mbar_wait_t(&a_full[sa], (ai / C::A_STAGES) & 1, w_m1)) { atomicExch(P.error_flag, 13u); ok = false; break; }
-          const uint32_t a_hi = smem_u32(smA + sa * C::A_STAGE), a_lo = a_hi + C::A_PLANE;
-          // The issuing thread is the bottleneck of the few-channel layers (72..108 MMAs per 256-pixel tile): build the
-          // descriptors once per stage and add compile-time offsets (the address field is (addr >> 4) in the low
-          // 14 bits; shared memory ends below 256 KB, so the addition never carries out of it).
-          const uint64_t dA_hi = make_desc_sw64(a_hi, 0), dA_lo = make_desc_sw64(a_lo, 0);
-#pragma unroll 1
-          for (int tap = 0; tap < 9; ++tap, ++bi) {
-            const uint32_t bgi = bi / C::BG, gs = bgi % RG;            // ring mode: group index and its slot group
-            const uint32_t sb = WRES ? (uint32_t)((cb * n_dz + dz) * 9 + tap) : gs * C::BG + bi % C::BG;
-            if (!WRES && bi % C::BG == 0) {
-              if (!mbar_wait_t(&b_full[gs], (bgi / RG) & 1, w_m2)) { atomicExch(P.error_flag, 14u); ok = false; break; }
-            }
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t dB_hi = make_desc_sw64(smem_u32(smB + (size_t)sb * C::B_STAGE), 0);
-            constexpr uint32_t B_LO = (uint32_t)(N * C::ROWB) >> 4;
-            const int dy = tap / 3, dx = tap % 3;
-#pragma unroll
-            for (int s = 0; s < S; ++s) {
-              const uint32_t roff = (uint32_t)((s + dy) * 130 + dx) * C::ROWB;
-              const uint32_t d = d0 + (uint32_t)(s * C::STRIP_COLS);
-#pragma unroll
-              for (int ks = 0; ks < C::KC / 16; ++ks) {
-                const uint32_t aoff = (roff + ks * 32) >> 4, boff = (uint32_t)(ks * 32) >> 4;
-                const uint64_t dah = dA_hi + aoff, dal = dA_lo + aoff, dbh = dB_hi + boff;
-                const uint32_t acc = (cbz | tap | ks) ? 1u : 0u;
-                if (C::MERGE) {
-                  if (elect_one()) umma_f16(d, dah, dbh, C::IDESC_2N, acc);       // [0,N): hi*Whi   [N,2N): hi*Wlo
-                  if (elect_one()) umma_f16(d + dsplit, dal, dbh, C::IDESC_N, 1u);   // lo*Whi -> [0,N), or [N,2N) with split_acc
-                } else {
-                  const uint64_t dbl = dbh + B_LO;
-                  if (elect_one()) umma_f16(d, dah, dbh, C::IDESC_N, acc);
-                  if (elect_one()) umma_f16(d, dal, dbh, C::IDESC_N, 1u);
-                  if (elect_one()) umma_f16(d, dah, dbl, C::IDESC_N, 1u);
-                }
-              }
-            }
-            if (!WRES && bi % C::BG == C::BG - 1 && elect_one()) tcgen05_commit(&b_empty[gs]);
-          }
-          if (!ok) break;
-          if (elect_one()) tcgen05_commit(&a_empty[sa]);
-        }
-        if (elect_one()) tcgen05_commit(&acc_full[buf]);
       }
-      if (P.dbg && lane == 0) { P.dbg[blockIdx.x * 8 + 0] = w_m0; P.dbg[blockIdx.x * 8 + 1] = w_m1; P.dbg[blockIdx.x * 8 + 2] = w_m2;
-                   P.dbg[blockIdx.x * 8 + 3] = (unsigned long long)(clock64() - t_m); }
+      wg_commit();
+      wg_wait<1>();                             // the previous stage's MMAs have retired: hand its slot back
+      if (kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % C::STAGES]);
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    uint32_t t = 0;
-    unsigned long long w_e = 0;
-    const long long t_e = clock64();
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t buf = t & 1;
-      const int img = tile / tiles_per_img, rem = tile - img * tiles_per_img;
-      const int y0 = (rem / tiles_x) * S, x = (rem % tiles_x) * 128 + m;
-      if (!mbar_wait_t(&acc_full[buf], (t >> 1) & 1, w_e)) {
-        atomicExch(P.error_flag, 15u);
-        if (FUSE) asm volatile("trap;");      // the fused epilogue meets at named barriers: abort rather than hang
-        break;
-      }
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tbase = tmem_base + ((uint32_t)(q * 32) << 16) + buf * (uint32_t)C::ACC_COLS;
-      if (FUSE) {
-        // features (bias + ReLU, fp32 straight from the accumulators) -> 1x1 heads on the CUDA cores -> prob / dist.
-        // The 128-channel feature map never goes to HBM (it was 512 MB written + 512 MB read per 1024^2 image).
-        // Eight epilogue warps; warps 2..5 compute dist 0..15, warps 6..9 dist 16..31 and prob, each for BOTH strips
-        // of its pixel column: one LDS.128 of head weights (shared memory, warp-wide broadcast) feeds 8 FFMAs.
-        // (Head weights in constant memory ran 5x slower: the 18 KB table misses the per-SMSP constant cache.)
-        const float* sHB = sHW;                      // [36] head biases
-        const float* sFB = sHW + 36;                 // [N] feature biases
-        const float* sW = sHW + 36 + N;              // [N][36] head weights
-        const uint32_t sFB_s = smem_u32(sFB), sW_s = smem_u32(sW);
-        const int grp = (warp - 2) >> 2;
+    wg_wait<0>();
+    wg_fence_regs<C::NREG>(acc); wg_fence_regs<C::NREG>(cor);
+    if (!ok) break;
+    if (n_kb > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % C::STAGES]);
+
+    // ---- epilogue: this thread holds pixels (y, x0 + lane/4) and (y, x0 + lane/4 + 8), channels c8*8 + (lane%4)*2 + {0,1}
+    const int y = by * 8 + wg * 4 + w;
+    const int xa = bx * 16 + (lane >> 2);
+    const int cq = (lane & 3) * 2;
+    if (FUSE) {
+      // features (bias + ReLU, fp32 straight from the accumulators) -> 1x1 heads on the CUDA cores -> prob / dist.
+      // The 128-channel feature map never goes to HBM.  Each thread sums its 32 channels of both pixels into the head
+      // outputs, the four threads of a quad (which together hold all 128 channels) reduce with shuffles.  Two passes
+      // over the outputs (dist 0..15, then dist 16..31 + prob) bound the live registers.
+      const uint32_t sFB_s = smem_u32(sHW + 36), sW_s = smem_u32(sHW + 36 + N);
+      // one accumulator from here on (the correction registers hold the constant 0 until the next tile's first MMA
+      // overwrites them), which keeps the head sums below the register budget
+#pragma unroll
+      for (int j = 0; j < C::NREG; ++j) { acc[j] += cor[j]; cor[j] = 0.f; }
+#pragma unroll
+      for (int grp = 0; grp < 2; ++grp) {
         float o0[17], o1[17];
 #pragma unroll
-        for (int o = 0; o < 16; ++o) { o0[o] = sHB[grp * 16 + o]; o1[o] = o0[o]; }
-        o0[16] = grp ? sHB[32] : 0.f; o1[16] = o0[16];
-#pragma unroll 1
-        for (int c0 = 0; c0 < N; c0 += 32) {
-          uint32_t r0[32], r1[32];
-          SDB_TMEM_LD32(r0, tbase + (uint32_t)c0);
-          SDB_TMEM_LD32(r1, tbase + (uint32_t)(C::STRIP_COLS + c0));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (c0 + 32 >= N) {
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-          }
+        for (int o = 0; o < 17; ++o) { o0[o] = 0.f; o1[o] = 0.f; }
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            // explicit ld.shared: the dynamic carve-up hides the address space from the compiler (generic LD.E otherwise)
-            const float fb = lds32(sFB_s + 4u * (uint32_t)(c0 + j));
-            float f0 = __uint_as_float(r0[j]) * P.acc_scale + fb, f1 = __uint_as_float(r1[j]) * P.acc_scale + fb;
+        for (int c8 = 0; c8 < N / 8; ++c8) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = c8 * 8 + cq + e;
+            const float fb = lds32(sFB_s + 4u * (uint32_t)c);
+            float f0 = acc[c8 * 4 + e] * P.acc_scale + fb;
+            float f1 = acc[c8 * 4 + 2 + e] * P.acc_scale + fb;
             if (P.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-            const uint32_t wrow = sW_s + 4u * (uint32_t)((c0 + j) * 36 + grp * 16);
+            const uint32_t wrow = sW_s + 4u * (uint32_t)(c * 36 + grp * 16);
 #pragma unroll
             for (int qq = 0; qq < 4; ++qq) {
-              const float4 w = lds128(wrow + 16u * qq);
-              o0[4 * qq] = fmaf(f0, w.x, o0[4 * qq]); o0[4 * qq + 1] = fmaf(f0, w.y, o0[4 * qq + 1]);
-              o0[4 * qq + 2] = fmaf(f0, w.z, o0[4 * qq + 2]); o0[4 * qq + 3] = fmaf(f0, w.w, o0[4 * qq + 3]);
-              o1[4 * qq] = fmaf(f1, w.x, o1[4 * qq]); o1[4 * qq + 1] = fmaf(f1, w.y, o1[4 * qq + 1]);
-              o1[4 * qq + 2] = fmaf(f1, w.z, o1[4 * qq + 2]); o1[4 * qq + 3] = fmaf(f1, w.w, o1[4 * qq + 3]);
+              const float4 wv = lds128(wrow + 16u * qq);
+              o0[4 * qq] = fmaf(f0, wv.x, o0[4 * qq]); o0[4 * qq + 1] = fmaf(f0, wv.y, o0[4 * qq + 1]);
+              o0[4 * qq + 2] = fmaf(f0, wv.z, o0[4 * qq + 2]); o0[4 * qq + 3] = fmaf(f0, wv.w, o0[4 * qq + 3]);
+              o1[4 * qq] = fmaf(f1, wv.x, o1[4 * qq]); o1[4 * qq + 1] = fmaf(f1, wv.y, o1[4 * qq + 1]);
+              o1[4 * qq + 2] = fmaf(f1, wv.z, o1[4 * qq + 2]); o1[4 * qq + 3] = fmaf(f1, wv.w, o1[4 * qq + 3]);
             }
-            if (grp) { const float w = lds32(sW_s + 4u * (uint32_t)((c0 + j) * 36 + 32)); o0[16] = fmaf(f0, w, o0[16]); o1[16] = fmaf(f1, w, o1[16]); }
+            if (grp) { const float wv = lds32(sW_s + 4u * (uint32_t)(c * 36 + 32)); o0[16] = fmaf(f0, wv, o0[16]); o1[16] = fmaf(f1, wv, o1[16]); }
           }
         }
 #pragma unroll
-        for (int s = 0; s < S; ++s) {
-          const int y = y0 + s;
-          const float* out = s ? o1 : o0;
-          if ((y < P.H) && (x < P.W)) {
-            const size_t pix = ((size_t)img * P.H + y) * P.W + x;
-            if (grp) P.prob[pix] = 1.f / (1.f + expf(-out[16]));
-            if (P.heads_R == 32) {
-              float4* d4 = reinterpret_cast<float4*>(P.dist + pix * 32 + grp * 16);
-#pragma unroll
-              for (int qq = 0; qq < 4; ++qq) d4[qq] = make_float4(out[4 * qq], out[4 * qq + 1], out[4 * qq + 2], out[4 * qq + 3]);
-            } else {
-#pragma unroll
-              for (int o = 0; o < 16; ++o) if (grp * 16 + o < P.heads_R) P.dist[pix * P.heads_R + grp * 16 + o] = out[o];
-            }
-          }
+        for (int o = 0; o < 17; ++o) {
+          o0[o] += __shfl_xor_sync(0xffffffffu, o0[o], 1); o0[o] += __shfl_xor_sync(0xffffffffu, o0[o], 2);
+          o1[o] += __shfl_xor_sync(0xffffffffu, o1[o], 1); o1[o] += __shfl_xor_sync(0xffffffffu, o1[o], 2);
         }
+        // quad thread q writes pixel q >> 1, outputs (q & 1) * 8 .. + 7 of this pass (and the prob)
+        const int q = lane & 3;
+        const int x = xa + ((q >> 1) ? 8 : 0);
+        if (y < P.H && x < P.W) {
+          const size_t pix = ((size_t)img * P.H + y) * P.W + x;
+          const int ob = grp * 16 + (q & 1) * 8;
+          float v[8];
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            const float a = (q & 1) ? o0[8 + k] : o0[k], b = (q & 1) ? o1[8 + k] : o1[k];
+            v[k] = ((q >> 1) ? b : a) + sHW[ob + k];
+          }
+          if (P.heads_R == 32) {
+            float4* d4 = reinterpret_cast<float4*>(P.dist + pix * 32 + ob);
+            d4[0] = make_float4(v[0], v[1], v[2], v[3]); d4[1] = make_float4(v[4], v[5], v[6], v[7]);
+          } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) if (ob + k < P.heads_R) P.dist[pix * P.heads_R + ob + k] = v[k];
+          }
+          if (grp && (q & 1) == 0) P.prob[pix] = 1.f / (1.f + expf(-(((q >> 1) ? o1[16] : o0[16]) + sHW[32])));
+        }
+      }
+      continue;
+    }
+    const float* bias = P.bias + nb * N;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int x = xa + 8 * h;
+      if (y >= P.H || x >= P.W) continue;
+      const size_t pix = ((size_t)img * P.H + y) * P.W + x;
+      if (P.heads_R > 0) {
+        // heads: channel 0 -> sigmoid -> prob, channels 1..R -> dist (fp32)
+#pragma unroll
+        for (int c8 = 0; c8 < N / 8; ++c8)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int ch = c8 * 8 + cq + e, j = c8 * 4 + 2 * h + e;
+            if (ch > P.heads_R) continue;
+            const float v = (acc[j] + cor[j]) * P.acc_scale + __ldg(bias + ch);
+            if (ch == 0) P.prob[pix] = 1.f / (1.f + expf(-v));
+            else P.dist[pix * P.heads_R + (ch - 1)] = v;
+          }
         continue;
       }
-#pragma unroll 1
-      for (int s = 0; s < S; ++s) {
-        const int y = y0 + s;
-        const bool in_img = (y < P.H) && (x < P.W);
-#pragma unroll 1
-        for (int c0 = 0; c0 < N; c0 += 32) {
-          uint32_t r[32];
-          SDB_TMEM_LD32(r, tbase + (uint32_t)(s * C::STRIP_COLS + c0));
-          if (C::MERGE) {
-            uint32_t r2[32];
-            SDB_TMEM_LD32(r2, tbase + (uint32_t)(s * C::STRIP_COLS + N + c0));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 #pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + __uint_as_float(r2[j]));
-          } else {
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          }
-          if (s == S - 1 && c0 + 32 >= N) {
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-          }
-          if (in_img) {
-            __align__(16) __half hi[32];
-            __align__(16) __half lo[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              float v = __uint_as_float(r[j]) * P.acc_scale + __ldg(P.bias + c0 + j);
-              if (P.relu) v = fmaxf(v, 0.f);
-              if (!(fabsf(v) <= 65504.f)) atomicOr(P.error_flag, 0x80000000u);
-              const __half h = __float2half_rn(v);
-              hi[j] = h;
-              lo[j] = __float2half_rn(v - __half2float(h));
-            }
-            if (!P.up2x) {
-              const size_t off = (((size_t)img * P.H + y) * P.W + x) * N + c0;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-                reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-              }
-            } else {
-              // nearest up-sampling written by the producer: 2x2 pixels, and both planes 2z, 2z+1 for a volume (up2x == 2)
-              const int H2 = 2 * P.H, W2 = 2 * P.W;
-              const int nrep = (P.up2x == 2) ? 8 : 4;
-#pragma unroll 1
-              for (int rep = 0; rep < nrep; ++rep) {
-                const size_t plane = (P.up2x == 2) ? (size_t)(2 * img + (rep >> 2)) : (size_t)img;
-                const size_t off = ((plane * H2 + (2 * y + ((rep >> 1) & 1))) * W2 + (2 * x + (rep & 1))) * N + c0;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  reinterpret_cast<uint4*>(P.out_hi + off)[j] = reinterpret_cast<const uint4*>(hi)[j];
-                  reinterpret_cast<uint4*>(P.out_lo + off)[j] = reinterpret_cast<const uint4*>(lo)[j];
-                }
-              }
-            }
+      for (int c8 = 0; c8 < N / 8; ++c8) {
+        const int ch = c8 * 8 + cq, j = c8 * 4 + 2 * h;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + ch));
+        float v0 = (acc[j] + cor[j]) * P.acc_scale + bb.x, v1 = (acc[j + 1] + cor[j + 1]) * P.acc_scale + bb.y;
+        if (P.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (!(fabsf(v0) <= 65504.f) || !(fabsf(v1) <= 65504.f)) atomicOr(P.error_flag, 0x80000000u);   // fp16 range of the hi plane exceeded (or NaN)
+        const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
+        const __half2 hi = __halves2half2(h0, h1);
+        const __half2 lo = __halves2half2(__float2half_rn(v0 - __half2float(h0)), __float2half_rn(v1 - __half2float(h1)));
+        const int oc = nb * N + ch;
+        if (!P.up2x) {
+          const size_t off = pix * P.c_out + oc;
+          *reinterpret_cast<__half2*>(P.out_hi + off) = hi;
+          *reinterpret_cast<__half2*>(P.out_lo + off) = lo;
+        } else {
+          // nearest up-sampling written by the producer: 2x2 pixels, and both planes 2z, 2z+1 for a volume (up2x == 2)
+          const int H2 = 2 * P.H, W2 = 2 * P.W;
+          const int nrep = (P.up2x == 2) ? 8 : 4;
+          for (int rep = 0; rep < nrep; ++rep) {
+            const size_t plane = (P.up2x == 2) ? (size_t)(2 * img + (rep >> 2)) : (size_t)img;
+            const size_t off = ((plane * H2 + (2 * y + ((rep >> 1) & 1))) * W2 + (2 * x + (rep & 1))) * P.c_out + oc;
+            *reinterpret_cast<__half2*>(P.out_hi + off) = hi;
+            *reinterpret_cast<__half2*>(P.out_lo + off) = lo;
           }
         }
       }
     }
-    if (P.dbg && threadIdx.x == 64) { P.dbg[blockIdx.x * 8 + 4] = w_e; P.dbg[blockIdx.x * 8 + 5] = (unsigned long long)(clock64() - t_e); }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)C::TMEM_COLS) : "memory");
   }
 }
 
@@ -1188,20 +666,6 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static int make_act_map2(CUtensorMap* m, const __half* base, int n, int h, int w, int c, int rows) {
-  // v2: box = {32 channels, 130 x, rows y, 1}, 64-byte swizzle
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { sdb::set_error("cuTensorMapEncodeTiled entry point not available"); return 1; }
-  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)w * c * 2, (cuuint64_t)h * w * c * 2};
-  cuuint32_t box[4] = {32, 130, (cuuint32_t)rows, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { sdb::set_error("cuTensorMapEncodeTiled(activation v2) failed: " + std::to_string((int)r)); return 1; }
-  return 0;
-}
-
 static int make_act_map(CUtensorMap* m, const __half* base, int n, int h, int w, int c, int kc) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { sdb::set_error("cuTensorMapEncodeTiled entry point not available"); return 1; }
@@ -1215,12 +679,13 @@ static int make_act_map(CUtensorMap* m, const __half* base, int n, int h, int w,
   if (r != CUDA_SUCCESS) { sdb::set_error("cuTensorMapEncodeTiled(activation) failed: " + std::to_string((int)r)); return 1; }
   return 0;
 }
-static int make_w_map(CUtensorMap* m, const __half* base, int cin, int cout, int kc, int n_taps = 9) {
+// weights [n_taps][cout][cin]; box = {kc, nbox output channels, 1 tap}
+static int make_w_map(CUtensorMap* m, const __half* base, int cin, int cout, int kc, int nbox, int n_taps) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { sdb::set_error("cuTensorMapEncodeTiled entry point not available"); return 1; }
   cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)cout, (cuuint64_t)n_taps};
   cuuint64_t strides[2] = {(cuuint64_t)cin * 2, (cuuint64_t)cin * cout * 2};
-  cuuint32_t box[3] = {(cuuint32_t)kc, (cuuint32_t)cout, 1};
+  cuuint32_t box[3] = {(cuuint32_t)kc, (cuuint32_t)nbox, 1};
   cuuint32_t es[3] = {1, 1, 1};
   const CUtensorMapSwizzle sw = (kc * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
@@ -1229,82 +694,70 @@ static int make_w_map(CUtensorMap* m, const __half* base, int cin, int cout, int
   return 0;
 }
 
-template <int N, int KC>
-static int launch_tc(const CUtensorMap& a0h, const CUtensorMap& a0l, const CUtensorMap& a1h, const CUtensorMap& a1l,
-                     const CUtensorMap& wh, const CUtensorMap& wl, const ConvParams& P, int n_img, cudaStream_t st) {
-  using C = TcCfg<N, KC>;
-  static bool attr = false;
-  if (!attr) { SDB_CUDA(cudaFuncSetAttribute(k_conv_tc<N, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM)); attr = true; }
-  dim3 grid(cdiv(P.W, 16), cdiv(P.H, 8), n_img);
-  sdb::ProfSpan sp;
-  sdb::profile_begin("conv_tc", st, &sp);
-  k_conv_tc<N, KC><<<grid, 192, C::SMEM, st>>>(a0h, a0l, a1h, a1l, wh, wl, P);
-  sdb::profile_end("conv_tc", st, &sp);
-  sdb::profile_add_units("conv_tc", 2.0 * P.n_taps * P.c_total * (P.heads_R > 0 ? P.heads_R + 1 : N) * (double)P.H * P.W * n_img);     // algorithmic FLOPs
-  sdb::g_launch_count++;
-  SDB_CUDA(cudaGetLastError());
-  return 0;
-}
-
 static int g_tc_split_acc = 1;   // see ConvParams::split_acc / sdb_tc_set_split_acc
-static int g_tc_variant = 0;      // 0 = auto (k_conv_tc4 for Cin <= 64, else k_conv_tc3, k_conv_tc for Cout = 256); 1 / 3 / 4 force a kernel where applicable
+static int g_tc_variant = 0;     // 0 = auto (persistent, 64-channel K blocks where the channel counts allow), 1 / 3 / 4: see sdb_tc_set_variant
 static int g_num_sms = 0;
-static int g_tc_no_resident = 0;   // tests: force the weight ring in k_conv_tc4
-
-template <int N, int KC>
-static int launch_tc3(const CUtensorMap& a0h, const CUtensorMap& a0l, const CUtensorMap& a1h, const CUtensorMap& a1l,
-                      const CUtensorMap& wh, const CUtensorMap& wl, const ConvParams& P, int n_img, cudaStream_t st) {
-  using C = TcCfg3<N, KC>;
-  static bool attr = false;
-  if (!attr) { SDB_CUDA(cudaFuncSetAttribute(k_conv_tc3<N, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM)); attr = true; }
-  if (!g_num_sms) { int dev = 0; SDB_CUDA(cudaGetDevice(&dev)); SDB_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev)); }
-  const int tiles_x = cdiv(P.W, 16), tiles_y = cdiv(P.H, 8);
-  const int n_tiles = tiles_x * tiles_y * n_img;
-  const int grid = std::min(n_tiles, g_num_sms);
-  sdb::ProfSpan sp;
-  sdb::profile_begin("conv_tc", st, &sp);
-  k_conv_tc3<N, KC><<<grid, 192, C::SMEM, st>>>(a0h, a0l, a1h, a1l, wh, wl, P, tiles_x, tiles_y, n_tiles);
-  sdb::profile_end("conv_tc", st, &sp);
-  sdb::profile_add_units("conv_tc", 2.0 * P.n_taps * P.c_total * (P.heads_R > 0 ? P.heads_R + 1 : N) * (double)P.H * P.W * n_img);
-  sdb::g_launch_count++;
-  SDB_CUDA(cudaGetLastError());
-  return 0;
-}
-
-template <int N, bool FUSE, bool WRES>
-static int launch_tc4_impl(const CUtensorMap& a0h, const CUtensorMap& a0l, const CUtensorMap& a1h, const CUtensorMap& a1l,
-                           const CUtensorMap& wh, const CUtensorMap& wl, const ConvParams& P, int n_img, cudaStream_t st, int n_dz) {
-  using C = TcCfg4<N>;
-  const int n_cb = P.c_total / C::KC;
-  const int n_b_slots = WRES ? 9 * n_dz * n_cb : C::B_STAGES;
-  const int smem = C::SMEM_FIXED + n_b_slots * C::B_STAGE + (FUSE ? (36 + N + N * 36) * 4 : 0);
-  if (smem > 227 * 1024) { sdb::set_error("conv_tc4: shared memory budget exceeded"); return 1; }
-  static int attr = 0;
-  if (attr < smem) { SDB_CUDA(cudaFuncSetAttribute((k_conv_tc4<N, FUSE, WRES>), cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr = smem; }
-  if (!g_num_sms) { int dev = 0; SDB_CUDA(cudaGetDevice(&dev)); SDB_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev)); }
-  const int tiles_x = cdiv(P.W, 128), tiles_y = cdiv(P.H, C::S);
-  const int n_tiles = tiles_x * tiles_y * n_img;
-  const int grid = std::min(n_tiles, g_num_sms);
-  sdb::ProfSpan sp;
-  sdb::profile_begin("conv_tc", st, &sp);
-  k_conv_tc4<N, FUSE, WRES><<<grid, FUSE ? 352 : 224, smem, st>>>(a0h, a0l, a1h, a1l, wh, wl, P, tiles_x, tiles_y, n_tiles, n_b_slots, n_dz);
-  sdb::profile_end("conv_tc", st, &sp);
-  sdb::profile_add_units("conv_tc", (2.0 * 9.0 * n_dz * P.c_total * N + (FUSE ? 2.0 * N * (P.heads_R + 1) : 0.0)) * (double)P.H * P.W * n_img);
-  sdb::g_launch_count++;
-  SDB_CUDA(cudaGetLastError());
-  return 0;
-}
-template <int N, bool FUSE = false>
-static int launch_tc4(const CUtensorMap& a0h, const CUtensorMap& a0l, const CUtensorMap& a1h, const CUtensorMap& a1l,
-                      const CUtensorMap& wh, const CUtensorMap& wl, const ConvParams& P, int n_img, cudaStream_t st, int n_dz = 1) {
-  using C = TcCfg4<N>;
-  const int n_cb = P.c_total / C::KC;
-  if (!FUSE && 9 * n_dz * n_cb * C::B_STAGE <= C::W_RESIDENT_MAX && !g_tc_no_resident)
-    return launch_tc4_impl<N, FUSE, true>(a0h, a0l, a1h, a1l, wh, wl, P, n_img, st, n_dz);
-  return launch_tc4_impl<N, FUSE, false>(a0h, a0l, a1h, a1l, wh, wl, P, n_img, st, n_dz);
-}
-
 static unsigned int* g_err_flag = nullptr;      // device flag shared by all launches
+
+template <int N, int KC, bool FUSE = false>
+static int launch_wg(const CUtensorMap& a0h, const CUtensorMap& a0l, const CUtensorMap& a1h, const CUtensorMap& a1l,
+                     const CUtensorMap& wh, const CUtensorMap& wl, const ConvParams& P, int n_img, cudaStream_t st) {
+  using C = WgCfg<N, KC, FUSE>;
+  static bool attr = false;
+  if (!attr) { SDB_CUDA(cudaFuncSetAttribute(k_conv_wg<N, KC, FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM)); attr = true; }
+  if (!g_num_sms) { int dev = 0; SDB_CUDA(cudaGetDevice(&dev)); SDB_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev)); }
+  const int tiles_x = cdiv(P.W, 16), tiles_y = cdiv(P.H, 8), n_nb = P.heads_R > 0 ? 1 : P.c_out / N;
+  const int n_tiles = tiles_x * tiles_y * n_nb * n_img;
+  const int grid = (g_tc_variant == 1) ? n_tiles : std::min(n_tiles, g_num_sms);
+  const int n_out = (P.heads_R > 0 && !FUSE) ? P.heads_R + 1 : P.c_out;
+  sdb::ProfSpan sp;
+  sdb::profile_begin("conv_tc", st, &sp);
+  k_conv_wg<N, KC, FUSE><<<grid, kThreads, C::SMEM, st>>>(a0h, a0l, a1h, a1l, wh, wl, P, tiles_x, tiles_y, n_nb, n_tiles);
+  sdb::profile_end("conv_tc", st, &sp);
+  sdb::profile_add_units("conv_tc", (2.0 * P.n_taps * P.c_total * n_out + (FUSE ? 2.0 * N * (P.heads_R + 1) : 0.0)) * (double)P.H * P.W * n_img);     // algorithmic FLOPs
+  sdb::g_launch_count++;
+  SDB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// activation maps of both sources and the weight maps for KC-channel blocks and N-channel output tiles
+static int make_conv_maps(CUtensorMap* a0h, CUtensorMap* a0l, CUtensorMap* a1h, CUtensorMap* a1l, CUtensorMap* wh, CUtensorMap* wl,
+                          const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo, int c_src1,
+                          int n, int h, int w, const void* w_hi, const void* w_lo, int cout, int kc, int nbox, int n_taps) {
+  if (make_act_map(a1h, (const __half*)src1_hi, n, h, w, c_src1, kc) || make_act_map(a1l, (const __half*)src1_lo, n, h, w, c_src1, kc)) return 1;
+  if (c_src0 > 0) {
+    if (make_act_map(a0h, (const __half*)src0_hi, n, h, w, c_src0, kc) || make_act_map(a0l, (const __half*)src0_lo, n, h, w, c_src0, kc)) return 1;
+  } else { *a0h = *a1h; *a0l = *a1l; }
+  const int cin = c_src0 + c_src1;
+  return make_w_map(wh, (const __half*)w_hi, cin, cout, kc, nbox, n_taps) || make_w_map(wl, (const __half*)w_lo, cin, cout, kc, nbox, n_taps);
+}
+
+// K block: 64 channels (128-byte swizzled rows) when both sources allow it, else 32; variant 4 forces 32, variant 3 forces 64 where possible
+static int pick_kc(int c_src0, int c_src1) {
+  const bool k64 = (c_src0 % 64 == 0) && (c_src1 % 64 == 0);
+  return (g_tc_variant == 4 || !k64) ? 32 : 64;
+}
+
+// 3x3 (n_taps 9) or 3x3x3 (n_taps 27) convolution, Cout in {32, 64, 128, 256} (256 = two 128-channel output tiles)
+static int conv_tc(const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo, int c_src1,
+                   int n, int h, int w, const void* w_hi, const void* w_lo, float w_scale, const float* d_bias, int cout, int relu,
+                   int up2x, void* out_hi, void* out_lo, int n_taps, cudaStream_t st) {
+  const int cin = c_src0 + c_src1;
+  if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
+  const int kc = pick_kc(c_src0, c_src1);
+  const int nt = std::min(cout, 128);
+  CUtensorMap a0h, a0l, a1h, a1l, wh, wl;
+  if (make_conv_maps(&a0h, &a0l, &a1h, &a1l, &wh, &wl, src0_hi, src0_lo, c_src0, src1_hi, src1_lo, c_src1, n, h, w, w_hi, w_lo, cout, kc, nt, n_taps))
+    return 1;
+  ConvParams P;
+  P.H = h; P.W = w; P.c_src0 = c_src0; P.c_total = cin; P.c_out = cout; P.relu = relu; P.up2x = up2x; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
+  P.out_hi = (__half*)out_hi; P.out_lo = (__half*)out_lo; P.error_flag = g_err_flag; P.n_taps = n_taps; P.heads_R = 0; P.prob = nullptr; P.dist = nullptr;
+  P.fuse_w = nullptr; P.fuse_b = nullptr; P.split_acc = g_tc_split_acc;
+#define SDB_WG(NN, KK) return launch_wg<NN, KK>(a0h, a0l, a1h, a1l, wh, wl, P, n, st)
+  if (kc == 64) { if (nt == 32) SDB_WG(32, 64); if (nt == 64) SDB_WG(64, 64); SDB_WG(128, 64); }
+  if (nt == 32) SDB_WG(32, 32); if (nt == 64) SDB_WG(64, 32); SDB_WG(128, 32);
+#undef SDB_WG
+}
 
 }  // namespace
 
@@ -1314,46 +767,10 @@ static unsigned int* g_err_flag = nullptr;      // device flag shared by all lau
 extern "C" int sdb_conv3x3_tc(const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo,
                               int c_src1, int n, int h, int w, const void* w_hi, const void* w_lo, float w_scale, const float* d_bias, int cout,
                               int relu, int up2x, void* out_hi, void* out_lo, sdb_stream_t stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  const int cin = c_src0 + c_src1;
-  const int kc = (cin % 64 == 0 && (c_src0 % 64 == 0)) ? 64 : 32;
-  if (cin % kc || c_src0 % kc || c_src1 % kc) { sdb::set_error("conv3x3_tc: channel counts must be multiples of 32"); return 1; }
+  if ((c_src0 + c_src1) % 32 || c_src0 % 32 || c_src1 % 32) { sdb::set_error("conv3x3_tc: channel counts must be multiples of 32"); return 1; }
   if (cout != 32 && cout != 64 && cout != 128 && cout != 256) { sdb::set_error("conv3x3_tc: cout must be 32/64/128/256"); return 1; }
-  if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
-  CUtensorMap a0h, a0l, a1h, a1l, wh, wl;
-  ConvParams P;
-  P.H = h; P.W = w; P.c_src0 = c_src0; P.c_total = cin; P.relu = relu; P.up2x = up2x; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
-  P.out_hi = (__half*)out_hi; P.out_lo = (__half*)out_lo; P.error_flag = g_err_flag; P.n_taps = 9; P.heads_R = 0; P.prob = nullptr; P.dist = nullptr; P.fuse_w = nullptr; P.fuse_b = nullptr; P.dbg = g_tc_dbg; P.split_acc = g_tc_split_acc;
-  if ((g_tc_variant == 4 || (g_tc_variant == 0 && cin <= 64 && w >= 96)) && cout <= 128) {
-    // halo-reuse persistent kernel: 32-channel blocks, (S+2) x 130 pixel boxes
-    constexpr int ROWS = TcCfg4<32>::S + 2;
-    if (make_act_map2(&a1h, (const __half*)src1_hi, n, h, w, c_src1, ROWS) || make_act_map2(&a1l, (const __half*)src1_lo, n, h, w, c_src1, ROWS)) return 1;
-    if (c_src0 > 0) {
-      if (make_act_map2(&a0h, (const __half*)src0_hi, n, h, w, c_src0, ROWS) || make_act_map2(&a0l, (const __half*)src0_lo, n, h, w, c_src0, ROWS)) return 1;
-    } else { a0h = a1h; a0l = a1l; }
-    if (make_w_map(&wh, (const __half*)w_hi, cin, cout, 32) || make_w_map(&wl, (const __half*)w_lo, cin, cout, 32)) return 1;
-    if (cout == 32) return launch_tc4<32>(a0h, a0l, a1h, a1l, wh, wl, P, n, st);
-    if (cout == 64) return launch_tc4<64>(a0h, a0l, a1h, a1l, wh, wl, P, n, st);
-    return launch_tc4<128>(a0h, a0l, a1h, a1l, wh, wl, P, n, st);
-  }
-  if (make_act_map(&a1h, (const __half*)src1_hi, n, h, w, c_src1, kc) || make_act_map(&a1l, (const __half*)src1_lo, n, h, w, c_src1, kc)) return 1;
-  if (c_src0 > 0) {
-    if (make_act_map(&a0h, (const __half*)src0_hi, n, h, w, c_src0, kc) || make_act_map(&a0l, (const __half*)src0_lo, n, h, w, c_src0, kc)) return 1;
-  } else { a0h = a1h; a0l = a1l; }
-  if (make_w_map(&wh, (const __half*)w_hi, cin, cout, kc) || make_w_map(&wl, (const __half*)w_lo, cin, cout, kc)) return 1;
-#define SDB_TC3(NN, KK) return launch_tc3<NN, KK>(a0h, a0l, a1h, a1l, wh, wl, P, n, st)
-  if ((g_tc_variant == 3 || g_tc_variant == 0 || g_tc_variant == 4) && cout <= 128) {
-    if (kc == 64) { if (cout == 32) SDB_TC3(32, 64); if (cout == 64) SDB_TC3(64, 64); SDB_TC3(128, 64); }
-    else { if (cout == 32) SDB_TC3(32, 32); if (cout == 64) SDB_TC3(64, 32); SDB_TC3(128, 32); }
-  }
-#undef SDB_TC3
-#define SDB_TC(NN, KK) return launch_tc<NN, KK>(a0h, a0l, a1h, a1l, wh, wl, P, n, st)
-  if (kc == 64) {
-    if (cout == 32) SDB_TC(32, 64); if (cout == 64) SDB_TC(64, 64); if (cout == 128) SDB_TC(128, 64); SDB_TC(256, 64);
-  } else {
-    if (cout == 32) SDB_TC(32, 32); if (cout == 64) SDB_TC(64, 32); if (cout == 128) SDB_TC(128, 32); SDB_TC(256, 32);
-  }
-#undef SDB_TC
+  return conv_tc(src0_hi, src0_lo, c_src0, src1_hi, src1_lo, c_src1, n, h, w, w_hi, w_lo, w_scale, d_bias, cout, relu, up2x ? 1 : 0,
+                 out_hi, out_lo, 9, (cudaStream_t)stream);
 }
 
 // 1x1 heads on the tensor cores: features [n,h,w,cfeat] (split fp16) x head weights [1][NP][cfeat] (split fp16,
@@ -1363,24 +780,18 @@ extern "C" int sdb_heads_tc(const void* f_hi, const void* f_lo, int cfeat, int n
   cudaStream_t st = (cudaStream_t)stream;
   if (cfeat % 64) { sdb::set_error("heads_tc: feature channels must be a multiple of 64"); return 1; }
   if (n_rays + 1 > np) { sdb::set_error("heads_tc: padded head count too small"); return 1; }
+  if (np != 48 && np != 80 && np != 112 && np != 144) { sdb::set_error("heads_tc: np must be one of 48, 80, 112, 144"); return 1; }
   if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
   CUtensorMap ah, al, wh, wl;
-  if (make_act_map(&ah, (const __half*)f_hi, n, h, w, cfeat, 64) || make_act_map(&al, (const __half*)f_lo, n, h, w, cfeat, 64)) return 1;
-  if (make_w_map(&wh, (const __half*)w_hi, cfeat, np, 64, 1) || make_w_map(&wl, (const __half*)w_lo, cfeat, np, 64, 1)) return 1;
+  if (make_conv_maps(&ah, &al, &ah, &al, &wh, &wl, nullptr, nullptr, 0, f_hi, f_lo, cfeat, n, h, w, w_hi, w_lo, np, 64, np, 1)) return 1;
   ConvParams P;
-  P.H = h; P.W = w; P.c_src0 = 0; P.c_total = cfeat; P.relu = 0; P.up2x = 0; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
-  P.out_hi = nullptr; P.out_lo = nullptr; P.error_flag = g_err_flag; P.n_taps = 1; P.heads_R = n_rays; P.prob = d_prob; P.dist = d_dist; P.fuse_w = nullptr; P.fuse_b = nullptr; P.dbg = nullptr; P.split_acc = g_tc_split_acc;
-  if (g_tc_variant != 1) {
-    if (np == 48) return launch_tc3<48, 64>(ah, al, ah, al, wh, wl, P, n, st);
-    if (np == 80) return launch_tc3<80, 64>(ah, al, ah, al, wh, wl, P, n, st);
-    if (np == 112) return launch_tc3<112, 64>(ah, al, ah, al, wh, wl, P, n, st);
-  }
-  if (np == 48) return launch_tc<48, 64>(ah, al, ah, al, wh, wl, P, n, st);
-  if (np == 80) return launch_tc<80, 64>(ah, al, ah, al, wh, wl, P, n, st);
-  if (np == 112) return launch_tc<112, 64>(ah, al, ah, al, wh, wl, P, n, st);
-  if (np == 144) return launch_tc<144, 64>(ah, al, ah, al, wh, wl, P, n, st);
-  sdb::set_error("heads_tc: np must be one of 48, 80, 112, 144");
-  return 1;
+  P.H = h; P.W = w; P.c_src0 = 0; P.c_total = cfeat; P.c_out = np; P.relu = 0; P.up2x = 0; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
+  P.out_hi = nullptr; P.out_lo = nullptr; P.error_flag = g_err_flag; P.n_taps = 1; P.heads_R = n_rays; P.prob = d_prob; P.dist = d_dist;
+  P.fuse_w = nullptr; P.fuse_b = nullptr; P.split_acc = g_tc_split_acc;
+  if (np == 48) return launch_wg<48, 64>(ah, al, ah, al, wh, wl, P, n, st);
+  if (np == 80) return launch_wg<80, 64>(ah, al, ah, al, wh, wl, P, n, st);
+  if (np == 112) return launch_wg<112, 64>(ah, al, ah, al, wh, wl, P, n, st);
+  return launch_wg<144, 64>(ah, al, ah, al, wh, wl, P, n, st);
 }
 
 // features conv (3x3, Cin <= 64 -> 128, bias, ReLU) fused with the 1x1 heads: prob = sigmoid(f . w_p + b_p),
@@ -1396,121 +807,39 @@ extern "C" int sdb_conv3x3_heads_tc(const void* src0_hi, const void* src0_lo, in
   if (n_rays < 1 || n_rays > 32) { sdb::set_error("conv3x3_heads_tc: n_rays must be in [1,32]"); return 1; }
   if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
   CUtensorMap a0h, a0l, a1h, a1l, wh, wl;
-  constexpr int ROWS = TcCfg4<128>::S + 2;
-  if (make_act_map2(&a1h, (const __half*)src1_hi, n, h, w, c_src1, ROWS) || make_act_map2(&a1l, (const __half*)src1_lo, n, h, w, c_src1, ROWS)) return 1;
-  if (c_src0 > 0) {
-    if (make_act_map2(&a0h, (const __half*)src0_hi, n, h, w, c_src0, ROWS) || make_act_map2(&a0l, (const __half*)src0_lo, n, h, w, c_src0, ROWS)) return 1;
-  } else { a0h = a1h; a0l = a1l; }
-  if (make_w_map(&wh, (const __half*)w_hi, cin, cout, 32) || make_w_map(&wl, (const __half*)w_lo, cin, cout, 32)) return 1;
+  if (make_conv_maps(&a0h, &a0l, &a1h, &a1l, &wh, &wl, src0_hi, src0_lo, c_src0, src1_hi, src1_lo, c_src1, n, h, w, w_hi, w_lo, cout, 32, cout, 9))
+    return 1;
   ConvParams P;
-  P.H = h; P.W = w; P.c_src0 = c_src0; P.c_total = cin; P.relu = relu; P.up2x = 0; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
+  P.H = h; P.W = w; P.c_src0 = c_src0; P.c_total = cin; P.c_out = cout; P.relu = relu; P.up2x = 0; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
   P.out_hi = nullptr; P.out_lo = nullptr; P.error_flag = g_err_flag; P.n_taps = 9; P.heads_R = n_rays; P.prob = d_prob; P.dist = d_dist;
-  P.fuse_w = d_heads_w; P.fuse_b = d_heads_b; P.dbg = g_tc_dbg; P.split_acc = g_tc_split_acc;
-  return launch_tc4<128, true>(a0h, a0l, a1h, a1l, wh, wl, P, n, st);
+  P.fuse_w = d_heads_w; P.fuse_b = d_heads_b; P.split_acc = g_tc_split_acc;
+  return launch_wg<128, 32, true>(a0h, a0l, a1h, a1l, wh, wl, P, n, st);
 }
 
-// 3x3x3 convolution of ONE volume [d,h,w,c] (split fp16 planes) on the tensor cores: k_conv_tc4 with the z planes as the
-// tensor map's image axis and 27 weight taps [27][cout][cin] (tap = dz*9 + dy*3 + dx).  up2x: 0 none, 2 = nearest 2x2x2.
+// 3x3x3 convolution of ONE volume [d,h,w,c] (split fp16 planes) on the tensor cores: the z planes are the tensor map's
+// image axis and the 27 weight taps [27][cout][cin] (tap = dz*9 + dy*3 + dx).  up2x: 0 none, 2 = nearest 2x2x2.
 extern "C" int sdb_conv3x3x3_tc(const void* src0_hi, const void* src0_lo, int c_src0, const void* src1_hi, const void* src1_lo,
                                 int c_src1, int d, int h, int w, const void* w_hi, const void* w_lo, float w_scale, const float* d_bias, int cout,
                                 int relu, int up2x, void* out_hi, void* out_lo, sdb_stream_t stream) {
-  cudaStream_t st = (cudaStream_t)stream;
   const int cin = c_src0 + c_src1;
   if (cin % 32 || c_src0 % 32 || c_src1 % 32) { sdb::set_error("conv3x3x3_tc: channel counts must be multiples of 32"); return 1; }
   if (cout != 32 && cout != 64 && cout != 128) { sdb::set_error("conv3x3x3_tc: cout must be 32/64/128"); return 1; }
   if (up2x != 0 && up2x != 2) { sdb::set_error("conv3x3x3_tc: up2x must be 0 or 2"); return 1; }
-  if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
-  CUtensorMap a0h, a0l, a1h, a1l, wh, wl;
-  constexpr int ROWS = TcCfg4<32>::S + 2;
-  if (make_act_map2(&a1h, (const __half*)src1_hi, d, h, w, c_src1, ROWS) || make_act_map2(&a1l, (const __half*)src1_lo, d, h, w, c_src1, ROWS)) return 1;
-  if (c_src0 > 0) {
-    if (make_act_map2(&a0h, (const __half*)src0_hi, d, h, w, c_src0, ROWS) || make_act_map2(&a0l, (const __half*)src0_lo, d, h, w, c_src0, ROWS)) return 1;
-  } else { a0h = a1h; a0l = a1l; }
-  if (make_w_map(&wh, (const __half*)w_hi, cin, cout, 32, 27) || make_w_map(&wl, (const __half*)w_lo, cin, cout, 32, 27)) return 1;
-  ConvParams P;
-  P.H = h; P.W = w; P.c_src0 = c_src0; P.c_total = cin; P.relu = relu; P.up2x = up2x; P.bias = d_bias; P.acc_scale = 1.0f / w_scale;
-  P.out_hi = (__half*)out_hi; P.out_lo = (__half*)out_lo; P.error_flag = g_err_flag; P.n_taps = 9; P.heads_R = 0; P.prob = nullptr; P.dist = nullptr; P.fuse_w = nullptr; P.fuse_b = nullptr; P.dbg = g_tc_dbg; P.split_acc = g_tc_split_acc;
-  if (cout == 32) return launch_tc4<32>(a0h, a0l, a1h, a1l, wh, wl, P, d, st, 3);
-  if (cout == 64) return launch_tc4<64>(a0h, a0l, a1h, a1l, wh, wl, P, d, st, 3);
-  return launch_tc4<128>(a0h, a0l, a1h, a1l, wh, wl, P, d, st, 3);
+  return conv_tc(src0_hi, src0_lo, c_src0, src1_hi, src1_lo, c_src1, d, h, w, w_hi, w_lo, w_scale, d_bias, cout, relu, up2x,
+                 out_hi, out_lo, 27, (cudaStream_t)stream);
 }
 
-// A/B switch for tests and profiling: 0 = auto (default), 1 = one tile per CTA, 3 = persistent, 4 = persistent + halo reuse
+// A/B switch for tests and profiling: 0 = auto (default), 1 = one tile per CTA (non-persistent grid),
+// 3 = persistent with 64-channel K blocks where the channel counts allow, 4 = persistent with 32-channel K blocks
 extern "C" int sdb_tc_set_variant(int variant) {
   if (variant != 0 && variant != 1 && variant != 3 && variant != 4) { sdb::set_error("tc_set_variant: 0 (auto), 1, 3 or 4"); return 1; }
   g_tc_variant = variant;
   return 0;
 }
 
-// ---------------------------------------------------------------------------------- TMA probe (profiling aid)
-// Persistent CTAs that only stream (rows x 130 pixel x box_c channel) halo boxes of an [n,h,w,c] fp16 tensor through
-// two shared-memory stages -- no MMA.  Measures what the TMA unit delivers for 64-byte vs 128-byte inner rows.
-__global__ void __launch_bounds__(64, 1) k_tma_probe(const __grid_constant__ CUtensorMap tm, int tiles_x, int tiles_y, int n_tiles, int rows,
-                                                     int stage_bytes, int box_bytes, int loads_per_tile, unsigned int* err) {
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + 2 * stage_bytes);
-  if (threadIdx.x == 0) {
-    mbar_init(&full[0], 1); mbar_init(&full[1], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int y0 = (tile / tiles_x) * (rows - 2), x0 = (tile % tiles_x) * 128;
-      const uint32_t s = it & 1;
-      if (it >= 2 && !mbar_wait(&full[s], ((it >> 1) - 1) & 1)) { atomicExch(err, 21u); break; }
-      mbar_expect_tx(&full[s], (uint32_t)(loads_per_tile * box_bytes));
-      for (int l = 0; l < loads_per_tile; ++l)
-        tma_load_4d(smem + s * stage_bytes + l * (((box_bytes + 1023) / 1024) * 1024), &tm, &full[s], 0, x0 - 1, y0 - 1, 0);
-    }
-    for (uint32_t k = (it >= 2 ? it - 2 : 0); k < it; ++k) mbar_wait(&full[k & 1], (k >> 1) & 1);
-  }
-}
-
-extern "C" int sdb_tma_probe(const void* d_act, int h, int w, int c, int box_c, int rows, int loads_per_tile, int reps, float* ms_out, sdb_stream_t stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  EncodeTiledFn enc = get_encode();
-  if (!enc) { sdb::set_error("cuTensorMapEncodeTiled entry point not available"); return 1; }
-  if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
-  CUtensorMap m;
-  cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, 1};
-  cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)w * c * 2, (cuuint64_t)h * w * c * 2};
-  cuuint32_t box[4] = {(cuuint32_t)box_c, 130, (cuuint32_t)rows, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  const CUtensorMapSwizzle sw = (box_c * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)d_act, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { sdb::set_error("tma_probe: cuTensorMapEncodeTiled failed: " + std::to_string((int)r)); return 1; }
-  const int box_bytes = box_c * 2 * 130 * rows;
-  const int stage_bytes = loads_per_tile * (((box_bytes + 1023) / 1024) * 1024);
-  const int smem = 2 * stage_bytes + 1024 + 64;
-  if (smem > 227 * 1024) { sdb::set_error("tma_probe: stage too large"); return 1; }
-  SDB_CUDA(cudaFuncSetAttribute(k_tma_probe, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  if (!g_num_sms) { int dev = 0; SDB_CUDA(cudaGetDevice(&dev)); SDB_CUDA(cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev)); }
-  const int tiles_x = cdiv(w, 128), tiles_y = cdiv(h, rows - 2), n_tiles = tiles_x * tiles_y;
-  cudaEvent_t e0, e1;
-  SDB_CUDA(cudaEventCreate(&e0)); SDB_CUDA(cudaEventCreate(&e1));
-  k_tma_probe<<<std::min(n_tiles, g_num_sms), 64, smem, st>>>(m, tiles_x, tiles_y, n_tiles, rows, stage_bytes, box_bytes, loads_per_tile, g_err_flag);
-  SDB_CUDA(cudaEventRecord(e0, st));
-  for (int i = 0; i < reps; ++i)
-    k_tma_probe<<<std::min(n_tiles, g_num_sms), 64, smem, st>>>(m, tiles_x, tiles_y, n_tiles, rows, stage_bytes, box_bytes, loads_per_tile, g_err_flag);
-  SDB_CUDA(cudaEventRecord(e1, st));
-  SDB_CUDA(cudaEventSynchronize(e1));
-  float ms = 0; SDB_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-  *ms_out = ms / reps;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  return 0;
-}
-
-// profiling aid: device buffer [148][8] of u64 that k_conv_tc4 launches fill with wait-cycle counters
-// (0 acc_empty, 1 a_full, 2 b_full, 3 MMA-warp total, 4 acc_full, 5 epilogue total, 6 a_empty), or NULL to disable
 extern "C" int sdb_tc_set_split_acc(int on) { g_tc_split_acc = on ? 1 : 0; return 0; }
-extern "C" int sdb_tc_set_debug(void* d_buf) { g_tc_dbg = (unsigned long long*)d_buf; return 0; }
 
-// non-zero when any tcgen05 conv launch since the last call hit a bounded-wait timeout (then results are invalid)
+// non-zero when any tensor-core conv launch since the last call hit a bounded-wait timeout (then results are invalid)
 extern "C" int sdb_tc_error_check(sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (!g_err_flag) return 0;
@@ -1519,8 +848,8 @@ extern "C" int sdb_tc_error_check(sdb_stream_t stream) {
   SDB_CUDA(cudaStreamSynchronize(st));
   if (v) {
     SDB_CUDA(cudaMemsetAsync(g_err_flag, 0, 4, st));
-    if (v & 0x7fffffffu) { sdb::set_error("tcgen05 conv: pipeline wait timed out (code " + std::to_string(v & 0x7fffffffu) + ")"); return 1; }
-    sdb::set_error("tcgen05 conv: fp16 overflow -- an activation exceeded 65504 (or is NaN) in the split-fp16 representation; normalise the input or use the fp32 CUDA-core path");
+    if (v & 0x7fffffffu) { sdb::set_error("tensor-core conv: pipeline wait timed out (code " + std::to_string(v & 0x7fffffffu) + ")"); return 1; }
+    sdb::set_error("tensor-core conv: fp16 overflow -- an activation exceeded 65504 (or is NaN) in the split-fp16 representation; normalise the input or use the fp32 CUDA-core path");
     return 2;
   }
   return 0;
@@ -1556,7 +885,7 @@ extern "C" int sdb_maxpool_split(const void* in_hi, const void* in_lo, int n, in
   cudaStream_t st = (cudaStream_t)stream;
   if ((h & 1) || (w & 1) || (c & 1)) { sdb::set_error("maxpool_split: needs even h, w, c"); return 1; }
   const long long total = (long long)n * (h / 2) * (w / 2) * (c / 2);
-  SDB_LAUNCH(k_maxpool_split, (int)std::min<long long>(cdiv(total, 256), 148 * 16), 256, 0, st, (const __half*)in_hi, (const __half*)in_lo, n, h, w, c,
+  SDB_LAUNCH(k_maxpool_split, (int)std::min<long long>(cdiv(total, 256), 132 * 16), 256, 0, st, (const __half*)in_hi, (const __half*)in_lo, n, h, w, c,
              (__half*)out_hi, (__half*)out_lo);
   return 0;
 }
@@ -1566,7 +895,7 @@ extern "C" int sdb_maxpool3d_split(const void* in_hi, const void* in_lo, int d, 
   cudaStream_t st = (cudaStream_t)stream;
   if (pz < 1 || py < 1 || px < 1 || d % pz || h % py || w % px || (c & 1)) { sdb::set_error("maxpool3d_split: sizes must be divisible by the pool, c even"); return 1; }
   const long long total = (long long)(d / pz) * (h / py) * (w / px) * (c / 2);
-  SDB_LAUNCH(k_maxpool3d_split, (int)std::min<long long>(cdiv(total, 256), 148 * 16), 256, 0, st, (const __half*)in_hi, (const __half*)in_lo, d, h, w, c,
+  SDB_LAUNCH(k_maxpool3d_split, (int)std::min<long long>(cdiv(total, 256), 132 * 16), 256, 0, st, (const __half*)in_hi, (const __half*)in_lo, d, h, w, c,
              pz, py, px, (__half*)out_hi, (__half*)out_lo);
   return 0;
 }
@@ -1574,7 +903,7 @@ extern "C" int sdb_split_f32(const float* d_in, long long n, void* out_hi, void*
   cudaStream_t st = (cudaStream_t)stream;
   if (!g_err_flag) { SDB_CUDA(cudaMalloc(&g_err_flag, 4)); SDB_CUDA(cudaMemset(g_err_flag, 0, 4)); }
   if (n <= 0) return 0;
-  SDB_LAUNCH(k_split_f32, (int)std::min<long long>(cdiv(n, 256), 148 * 32), 256, 0, st, d_in, n, (__half*)out_hi, (__half*)out_lo, g_err_flag);
+  SDB_LAUNCH(k_split_f32, (int)std::min<long long>(cdiv(n, 256), 132 * 32), 256, 0, st, d_in, n, (__half*)out_hi, (__half*)out_lo, g_err_flag);
   return 0;
 }
 

@@ -1,4 +1,4 @@
-"""StarDist2D on the B200 path.
+"""StarDist2D on the H100 path.
 
 Mirrors stardist/models/model2d.py: Config2D (:123-269, in config.py), StarDist2D._build
 (:310-349 -> UNetDevice2D), _instances_from_prediction (:512-563), _axes_div_by (:566-574).

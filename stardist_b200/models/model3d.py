@@ -1,4 +1,4 @@
-"""StarDist3D on the B200 path.
+"""StarDist3D on the H100 path.
 
 Mirrors stardist/models/model3d.py: Config3D (:129-311, in config.py), StarDist3D._build_unet
 (:360-399 -> UNetDeviceND), _instances_from_prediction (:589-674), _axes_div_by (:677-691).
@@ -30,7 +30,7 @@ class StarDist3D(StarDistBase):
         self.config.backbone == 'unet' or _raise(NotImplementedError(self.config.backbone))
         import os
         if os.environ.get("STARDIST_B200_UNET", "tc") != "simt" and UNetDevice3DTC.supported(self.config):
-            return UNetDevice3DTC(self.config, self.weights)      # tcgen05 3x3x3 convolutions
+            return UNetDevice3DTC(self.config, self.weights)      # tensor-core 3x3x3 convolutions
         return UNetDeviceND(self.config, self.weights)
 
     def _finish_labels(self, labels, overlap_label):

@@ -191,9 +191,9 @@ def tc_weight_scale(k):
 
 
 class UNetDevice2DTC:
-    """tcgen05 / TMA / TMEM executor (csrc/unet_tc.cu).  Activations are [2, N, H, W, C] float16
+    """wgmma / TMA executor (csrc/unet_tc.cu).  Activations are [2, N, H, W, C] float16
     tensors (plane 0 = hi, plane 1 = lo, value = hi + lo); convolutions run as three fp16 tensor-core
-    passes with fp32 accumulation in TMEM.  The Cin<=4 stem, 2x2 max-pooling and the 1x1 heads are
+    passes with fp32 accumulation in registers.  The Cin<=4 stem, 2x2 max-pooling and the 1x1 heads are
     small CUDA-core kernels on the same split format; nearest up-sampling is written by the
     producing convolution's epilogue."""
 
@@ -352,8 +352,8 @@ class UNetDevice2DTC:
 
 
 class UNetDevice3DTC:
-    """tcgen05 executor of the 3-D U-Net (model3d.py:360-399) for ONE volume: activations are [2, D, H, W, C] float16
-    planes (hi, lo); every 3x3x3 convolution with Cin % 32 == 0 runs on sdb_conv3x3x3_tc (k_conv_tc4: z planes as the
+    """tensor-core executor of the 3-D U-Net (model3d.py:360-399) for ONE volume: activations are [2, D, H, W, C] float16
+    planes (hi, lo); every 3x3x3 convolution with Cin % 32 == 0 runs on sdb_conv3x3x3_tc (k_conv_wg: z planes as the
     tensor map's image axis, 27 taps), the Cin <= 4 stem on the CUDA-core kernel followed by sdb_split_f32, pooling on
     sdb_maxpool3d_split, nearest 2x2x2 up-sampling written by the producing convolution, the 1x1x1 heads on the
     tensor-core heads kernel over the volume viewed as a [D*H, W] image."""

@@ -13,7 +13,7 @@ import numpy as np
 
 def build_parser():
     p = argparse.ArgumentParser(formatter_class=argparse.ArgumentDefaultsHelpFormatter,
-                                description="Prediction script for a stardist model folder on the B200 path")
+                                description="Prediction script for a stardist model folder on the H100 path")
     p.add_argument("-i", "--input", type=str, nargs="+", required=True, help="input file (tiff)")
     p.add_argument("-o", "--outdir", type=str, default=".", help="output directory")
     p.add_argument("--outname", type=str, default="{img}.stardist.tif", help="output file name (tiff)")

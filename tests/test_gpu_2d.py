@@ -1,4 +1,4 @@
-"""GPU parity tests of the 2D path (run on the B200 box: pytest -m gpu).  Everything goes through
+"""GPU parity tests of the 2D path (run on the H100 box: pytest -m gpu).  Everything goes through
 the C ABI of libstardist_b200.so; the checker is the oracle (reference C++ in oracle/_ref, numpy
 restatements) and the committed golden vectors.  Integer/index results must be bit-exact."""
 import os, sys
@@ -193,7 +193,7 @@ def test_predict_n_tiles_equals_untiled(sd, shape, n_tiles):
     p1, d1 = model.predict(img)
     p2, d2 = model.predict(img, n_tiles=n_tiles)
     assert p1.shape == p2.shape == shape and d1.shape == d2.shape
-    # same per-pixel arithmetic, but small tiles may pick a different tcgen05 kernel variant (summation order):
+    # same per-pixel arithmetic, but small tiles may pick a different tensor-core kernel variant (summation order):
     # equal to the float tolerance of the maps, not bitwise
     assert np.max(np.abs(p1 - p2)) <= 1e-5 * max(1.0, np.max(np.abs(p1)))
     assert np.max(np.abs(d1 - d2)) <= 1e-5 * max(1e-3, np.max(np.abs(d1))) + 1e-7
@@ -234,7 +234,7 @@ def test_reference_2d_demo_model_reproduces_reference_test(sd):
     ex_labels, ex = pipeline2d.predict_instances(cfg, weights, x, thr['prob'], thr['nms'], cand_from=model)
     assert np.array_equal(polygons2['points'], ex['points']) and np.array_equal(polygons2['prob'], ex['prob'])
     assert np.array_equal(polygons2['coord'].view(np.int32), ex['coord'].view(np.int32)) and np.array_equal(labels2, ex_labels)
-    # float maps of the TRAINED network (tcgen05 path) against a float64 evaluation: the 1e-5 relative bar
+    # float maps of the TRAINED network (tensor-core path) against a float64 evaluation: the 1e-5 relative bar
     import torch
     prob1, dist1 = model.predict(x)
     rp64, rd64 = unet_torch.forward(cfg, weights, x[None, ..., None].astype(np.float32), dtype=torch.float64)

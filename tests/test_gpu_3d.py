@@ -226,7 +226,7 @@ def test_multiclass_head_3d(sd):
 @pytest.mark.parametrize("d,h,w,c0,c1,cout,relu,up2x", [(5, 12, 40, 0, 32, 32, 1, 0), (4, 9, 130, 0, 64, 64, 1, 0), (3, 6, 20, 32, 32, 32, 0, 0),
                                                         (4, 8, 16, 0, 64, 32, 1, 2), (6, 10, 24, 0, 32, 128, 1, 0), (2, 5, 200, 64, 64, 64, 1, 0)])
 def test_conv3x3x3_tc_single_layer(d, h, w, c0, c1, cout, relu, up2x):
-    """tcgen05 3x3x3 convolution (z planes as the tensor map's image axis, 27 taps) vs a float64 conv3d of the same split
+    """tensor-core 3x3x3 convolution (z planes as the tensor map's image axis, 27 taps) vs a float64 conv3d of the same split
     operands; two-source (concat) inputs and the 2x2x2 up-sampling epilogue"""
     import torch, torch.nn.functional as F
     from stardist_b200 import _lib as L
@@ -260,7 +260,7 @@ def test_conv3x3x3_tc_single_layer(d, h, w, c0, c1, cout, relu, up2x):
 
 def test_unet3d_tc_vs_torch_fp32(sd):
     """3-D U-Net on the tensor cores against a float64 evaluation.  prob: 3e-7 of its scale.  dist of a RANDOM-INIT net is a
-    near-cancelling sum (max ~0.07 from O(1) features): the split-fp16 / TMEM-accumulated path leaves ~6e-7 absolute, i.e.
+    near-cancelling sum (max ~0.07 from O(1) features): the split-fp16 / register-accumulated path leaves ~6e-7 absolute, i.e.
     7e-6 of that tiny scale with split_acc (1.2e-5 without; tests/tools/tc_split_error.py, DESIGN.md 5) -- the bound is
     1e-5 of max(map scale, feature scale 1) and 2e-5 of the map scale itself."""
     import torch
@@ -361,8 +361,7 @@ def test_reference_nms_accuracy_property(sd, noise, n_rays):
     as there): rendered IoU of two polyhedra, NMS at 0.95*iou keeps one, at 1.05*iou keeps both.  With oracle/_ref the rendered
     masks are compared with the reference's: the polar rays of the golden spiral get dist == 10.0 exactly here (sin(2 pi * +-1),
     sin(0)), so each polyhedron has vertices ON the voxel lattice -- the documented hull-facet caveat (DESIGN.md 5, 3D labels:
-    the reference ANDs a Qhull hull test whose last-bit plane rounding decides such a voxel).  Measured on B200: exactly one
-    voxel of 2.9-5.1 k differs in 8 of the 12 cases, none in the others; the bound asserted here is 0.1 % (these polyhedra have radius ~10)."""
+    the reference ANDs a Qhull hull test whose last-bit plane rounding decides such a voxel).  The bound asserted here is 0.1 % (these polyhedra have radius ~10)."""
     from stardist_b200.geometry.geom3d import polyhedron_to_label
     from stardist_b200.nms import non_maximum_suppression_3d_sparse
     dist, points, prob, rays, shape = cases.nms3d_accuracy_inputs(noise, n_rays)

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 convolution path (csrc/unet_tc.cu): single layers against a float64
+"""GPU tests of the wgmma convolution path (csrc/unet_tc.cu): single layers against a float64
 torch convolution of the *same split operands*, then the whole network against torch-CPU fp32."""
 import os, sys
 import numpy as np
@@ -108,7 +108,7 @@ def test_unet_tc_head_variants(n_rays, fuse, monkeypatch):
 
 @pytest.mark.parametrize("variant", [1, 3, 4])
 def test_conv_variants_agree(variant):
-    """the three tcgen05 conv kernels (one tile per CTA / persistent / persistent + halo reuse) on one layer"""
+    """the conv kernel variants (one tile per CTA / persistent, 64-channel K blocks / persistent, 32-channel K blocks) on one layer"""
     import torch
     from stardist_b200 import _lib as L
     from stardist_b200.models.unet_device import tc_weight_scale

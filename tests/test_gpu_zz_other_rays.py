@@ -3,10 +3,9 @@
 Status: the arithmetic is pinned on the CPU (tests/test_cpu_oracle.py::test_serial_nms3d_other_ray_classes_equal_reference:
 host build of the device headers == reference extension, 0 decisions differ).  The DEVICE handling of coincident ray
 directions (Rays_Cartesian's pole rings: duplicate vertices -> sd3::demote_duplicate_points before the warp gift wrapping;
-zero-area pole faces listed in every direction bin) was written after this round's GPU budget was spent: it compiles for
-sm_100a and is the same header code as the host build, but it has not run on a GPU yet -- nor have Octo / Tetra ray sets,
-although they take the regular device path.  The whole file is therefore marked xfail(strict=False): a pass shows up as
-XPASS, a failure does not turn the suite red before anybody has looked at it."""
+zero-area pole faces listed in every direction bin) is the same header code as the host build.  On the H100 the Octo / Tetra
+NMS cases and the rendering of all three ray classes equal the reference; the Rays_Cartesian NMS test stays
+xfail(strict=False) because one of its cases (noise 0: equal distances on the pole rings) still differs -- an open defect."""
 import os, sys
 import numpy as np
 import pytest
@@ -15,8 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
 from oracle import ref_ext
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.xfail(strict=False, reason="written after the round's GPU budget was spent: CPU-pinned, compiled, not yet run on a GPU")]
+pytestmark = pytest.mark.gpu
 
 
 def _cloud(rays, noise, seed, n=300):
@@ -48,6 +46,8 @@ def test_device_nms3d_octo_tetra_vs_reference(cls, arg, noise, nthr):
     _run(getattr(R3, cls)(arg), noise, nthr, 7 + arg)
 
 
+@pytest.mark.xfail(strict=False, reason="open defect: on the H100 the device keeps different candidates than the reference for "
+                                        "[0.0-0.3-8-5] (equal distances on the pole rings) in every run so far; the other cases pass")
 @pytest.mark.parametrize("nx,nz", [(8, 5), (11, 5)])
 @pytest.mark.parametrize("noise,nthr", [(0.2, 0.2), (0.5, 0.5), (0.0, 0.3)])
 def test_device_nms3d_cartesian_vs_reference(nx, nz, noise, nthr):

@@ -1,7 +1,17 @@
 """Host-side formats either side of the path: ImageJ ROI export, TIFF in/out, the command line parser."""
-import ast, hashlib, os, zipfile
+import hashlib, os, zipfile
 import numpy as np
 import pytest
+
+
+def _golden():
+    """seeded inputs and the reference's outputs on them (sha256), frozen by tests/golden/make_io_ref.py"""
+    import json, sys
+    golden = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+    sys.path.insert(0, golden)
+    import io_cases
+    with open(os.path.join(golden, "io_ref.json")) as f:
+        return io_cases, json.load(f)
 
 
 def test_polyroi_bytes_golden_and_reference():
@@ -10,20 +20,10 @@ def test_polyroi_bytes_golden_and_reference():
     b = bytes(rois.polyroi_bytearray(x, y, pos=2, subpixel=True))
     assert len(b) == 112 and b[:4] == b"Iout"
     assert hashlib.sha256(b).hexdigest() == "9e394be9b5d3ae592c63d1bd595a585848eff9eca31af44bf83dc8026b2b4719"
-    ref_src = "/root/reference/stardist/utils.py"
-    if not os.path.exists(ref_src):
-        return
-    # the reference's function, compiled in isolation (its module imports csbdeep / skimage, which are not installed)
-    fn = [n for n in ast.parse(open(ref_src).read()).body if isinstance(n, ast.FunctionDef) and n.name == "polyroi_bytearray"][0]
-    ns = {"np": np}
-    exec(compile(ast.Module(body=[fn], type_ignores=[]), "ref_utils", "exec"), ns)
-    rng = np.random.default_rng(0)
-    for _ in range(25):
-        n = int(rng.integers(3, 40)); xs = rng.uniform(-5, 300, n); ys = rng.uniform(0, 200, n)
-        for sub in (True, False):
-            for pos in (None, 3):
-                assert bytes(rois.polyroi_bytearray(xs, ys, pos=pos, subpixel=sub)) == bytes(ns["polyroi_bytearray"](xs, ys, pos=pos, subpixel=sub))
-
+    # the reference's own function on the seeded cases, frozen by tests/golden/make_io_ref.py
+    cases, ref = _golden()
+    got = [hashlib.sha256(bytes(rois.polyroi_bytearray(xs, ys, pos=pos, subpixel=sub))).hexdigest() for xs, ys, pos, sub in cases.roi_cases()]
+    assert got == ref["polyroi_bytearray"]
 
 def test_export_imagej_rois_and_tiff_roundtrip(tmp_path):
     from stardist_b200.io import rois, tiff
@@ -51,7 +51,7 @@ def test_cli_parser():
 
 
 def test_export_to_obj_file3D(tmp_path):
-    """text identical to stardist/geometry/geom3d.py:277-347 (compiled in isolation where the reference tree is mounted)"""
+    """text identical to stardist/geometry/geom3d.py:277-347 (its outputs frozen in tests/golden/io_ref.json)"""
     import stardist_b200 as sd
     from stardist_b200.io import obj
     rays = sd.Rays_GoldenSpiral(12)
@@ -63,11 +63,6 @@ def test_export_to_obj_file3D(tmp_path):
     assert text.count("\nv ") + text.startswith("v ") == 4 * 12 and text.count("f ") == 4 * len(rays.faces) and text.startswith("o poly_0\n")
     with pytest.raises(ValueError):
         obj.export_to_obj_file3D(dict(dist=polys["dist"]))
-    ref_src = "/root/reference/stardist/geometry/geom3d.py"
-    if not os.path.exists(ref_src):
-        return
-    fns = [n for n in ast.parse(open(ref_src).read()).body if isinstance(n, ast.FunctionDef) and n.name in ("dist_to_coord3D", "export_to_obj_file3D")]
-    ns = {"np": np, "tqdm": (lambda x: x)}
-    exec(compile(ast.Module(body=fns, type_ignores=[]), "ref_geom3d", "exec"), ns)
-    for kw in (dict(), dict(single_mesh=False), dict(uv_map=True, scale=(2, 1, 0.5)), dict(scale=0.01)):
-        assert obj.export_to_obj_file3D(polys, **kw) == ns["export_to_obj_file3D"](dict(polys), **kw)
+    cases, ref = _golden()
+    got = [hashlib.sha256(obj.export_to_obj_file3D(cases.obj_polys(), **kw).encode()).hexdigest() for kw in cases.OBJ_KWARGS]
+    assert got == ref["export_to_obj_file3D"]

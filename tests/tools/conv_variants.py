@@ -1,4 +1,4 @@
-"""the three tcgen05 conv kernels (one tile per CTA / persistent / persistent + halo reuse) against a float64 convolution of
+"""the conv kernel variants (one tile per CTA / persistent, 64-channel K blocks / persistent, 32-channel K blocks) against a float64 convolution of
 the same split operands, and their timings on the layer shapes of the 1024x1024 forward pass"""
 import sys, os, time
 import numpy as np, torch, torch.nn.functional as F

@@ -1,6 +1,6 @@
 """configs[2] at full size (SURVEY 8d: 128x512x512, Rays_GoldenSpiral n_rays = 96, default Config3D), one GPU.
 
-R1 "network-real": the random-init 3-D U-Net (tcgen05 3x3x3 convolutions) on a synthetic volume, timed with CUDA events,
+R1 "network-real": the random-init 3-D U-Net (tensor-core 3x3x3 convolutions) on a synthetic volume, timed with CUDA events,
     then predict_instances end to end (host volume in, label volume out) with prob_thresh at a high quantile of its own
     prob map (a random-init dist head gives tiny polyhedra, so this exercises network + threshold/sort/gather + a trivial NMS).
 R2 "post-proc-real": candidates (prob, dist rows, points) derived analytically from ground-truth ellipsoids generated for a

@@ -51,13 +51,13 @@ for split in (0, 1):
     lib.sdb_tc_set_split_acc(split)
     model = sd.StarDist2D(cfg, name=None, basedir=None, weights=weights)
     prob, dist = model.predict(x)
-    errs("2D_demo tcgen05 split_acc=%d" % split, prob, dist, rp64, rd64)
+    errs("2D_demo tensor-core split_acc=%d" % split, prob, dist, rp64, rd64)
     model = sd.StarDist2D(cfg_b, name=None, basedir=None, weights=w_b)
     prob, dist = model.predict(img_b)
-    errs("bench net tcgen05 split_acc=%d" % split, prob, dist, bp64, bd64)
+    errs("bench net tensor-core split_acc=%d" % split, prob, dist, bp64, bd64)
     xc = torch.from_numpy(vol[None, ..., None]).cuda()
     p, d = m_c.net.forward(xc)
-    errs("3D random tcgen05 split_acc=%d" % split, p.cpu().numpy()[0], d.cpu().numpy()[0], cp64[0], cd64[0])
+    errs("3D random tensor-core split_acc=%d" % split, p.cpu().numpy()[0], d.cpu().numpy()[0], cp64[0], cd64[0])
     # speed of the bench forward with this setting
     xb = torch.from_numpy(bench_data.synthetic_image((1024, 1024), seed=0)[0][None, ..., None]).cuda()
     mb = sd.StarDist2D(cfg_b, name=None, basedir=None, weights=w_b)

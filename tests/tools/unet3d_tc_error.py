@@ -19,6 +19,6 @@ for shape, grid in (((16, 32, 48), (1, 1, 1)), ((8, 24, 136), (1, 2, 2))):
     for name, got, simt, r64, r32 in (("prob", prob, ps, rp64, rp32), ("dist", dist, ds, rd64, rd32)):
         g = got.cpu().numpy().astype(np.float64); s = simt.cpu().numpy().astype(np.float64)
         scale = float(np.max(np.abs(r64)))
-        print(shape, grid, name, "scale %.4g | tcgen05 %.3g | cuda-core fp32 %.3g | torch-cpu fp32 %.3g  (max abs error vs float64; relative to scale: %.2e / %.2e / %.2e)" %
+        print(shape, grid, name, "scale %.4g | tensor-core %.3g | cuda-core fp32 %.3g | torch-cpu fp32 %.3g  (max abs error vs float64; relative to scale: %.2e / %.2e / %.2e)" %
               (scale, np.max(np.abs(g - r64)), np.max(np.abs(s - r64)), np.max(np.abs(r32 - r64)),
                np.max(np.abs(g - r64)) / scale, np.max(np.abs(s - r64)) / scale, np.max(np.abs(r32 - r64)) / scale))
