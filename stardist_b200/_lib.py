@@ -209,8 +209,20 @@ class UNetConfigC(ctypes.Structure):
 
 def c_unet_create(config, weights):
     """network object of the C boundary (_LIB_unet_forward_2d/3d) from a Config2D/3D and a weights dict; returns
-    (handle, config struct).  The kernels are handed over in the order the library names the layers."""
+    (handle, config struct).  The kernels are handed over in the order the library names the layers.
+    sdb_unet_config has no fields for activations, batch norm, kernel size or pooling: the C executor always runs ReLU,
+    3^d kernels and 2^d pooling without batch norm, so any other config is refused here rather than run as a different net."""
     import numpy as np
+    unsupported = [(k, getattr(config, k)) for k in ("unet_activation", "unet_last_activation") if getattr(config, k) != 'relu']
+    if config.unet_batch_norm:
+        unsupported.append(("unet_batch_norm", config.unet_batch_norm))
+    if any(int(k) != 3 for k in config.unet_kernel_size):
+        unsupported.append(("unet_kernel_size", tuple(config.unet_kernel_size)))
+    if any(int(p) != 2 for p in config.unet_pool):
+        unsupported.append(("unet_pool", tuple(config.unet_pool)))
+    if unsupported:
+        raise StarDistB200Error("the C executor runs ReLU, 3^d kernels, pool 2 and no batch norm only; unsupported: %s"
+                                % ", ".join("%s=%r" % kv for kv in unsupported))
     lib = require_cuda()
     g = tuple(config.grid) + (1,) * (3 - len(config.grid))
     cfg = UNetConfigC(config.n_dim, config.n_channel_in, config.n_rays, config.unet_n_depth, config.unet_n_filter_base,
