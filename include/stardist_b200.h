@@ -146,6 +146,15 @@ int sdb_nms3d_set_split(int on);
 int sdb_relabel_sequential(int* d_labels, long long n, int max_label, int offset, int* d_forward_map,
                            int* h_count, sdb_stream_t stream);
 
+/* sparse label-overlap table (stardist/matching.py:38-52, _label_overlap): every distinct pair (a, b) = (d_a[i], d_b[i]) of
+ * two int32 label maps of n pixels / voxels, background 0 included, with its pixel count, sorted by (a, b).  Results go to
+ * d_pairs[capacity][2] (int32 a, b) and d_counts[capacity] (int64); *h_n_pairs = number of pairs, after one stream
+ * synchronisation.  When the pairs do not fit in `capacity`, nothing is written and *h_n_pairs > capacity is returned: an
+ * upper bound of the number of distinct pairs, so the caller can retry once with that capacity.  Negative labels are an
+ * error (matching.py:27-35).  capacity in [1, 2^28]: maps with more than 2^28 distinct pairs are not supported. */
+int sdb_label_overlap(const int* d_a, const int* d_b, long long n, int* d_pairs, long long* d_counts,
+                      long long capacity, long long* h_n_pairs, sdb_stream_t stream);
+
 /* 3D NMS on device arrays (see _LIB_non_maximum_suppression_sparse); d_keep is uint8[n_polys]. */
 int sdb_nms3d(const float* d_dist, const float* d_points, const float* d_verts, const int* d_faces,
               int n_polys, int n_rays, int n_faces, float threshold, int use_bbox, int use_kdtree,

@@ -86,6 +86,8 @@ def _declare(lib):
     lib.sdb_nms3d_set_variant.restype = c_int
     lib.sdb_relabel_sequential.argtypes = [P, c_longlong, c_int, c_int, P, POINTER(c_int), P]
     lib.sdb_relabel_sequential.restype = c_int
+    lib.sdb_label_overlap.argtypes = [P, P, c_longlong, P, P, c_longlong, POINTER(c_longlong), P]
+    lib.sdb_label_overlap.restype = c_int
     lib.sdb_nms3d.argtypes = [P, P, P, P, c_int, c_int, c_int, c_float, c_int, c_int, c_int, P, P]
     lib.sdb_unet_layer_count.argtypes = [P]
     lib.sdb_unet_layer_count.restype = c_int

@@ -13,11 +13,13 @@
 #include <vector>
 #include <algorithm>
 #include "common.cuh"
+#include "bitonic.cuh"
 #include "../../include/stardist_b200.h"
 
 namespace {
 
 using sdb::cdiv;
+using sdb::bitonic::BTILE;
 typedef unsigned long long u64;
 
 struct ShapeDesc {
@@ -42,68 +44,6 @@ __global__ void k_threshold(const float* __restrict__ prob, long long npix, Shap
     const unsigned int pos = atomicAdd(count, 1u);
     if (pos < capacity) keys[pos] = ((u64)sdb::float_order_key(v) << 32) | (u64)(unsigned int)p;
   }
-}
-
-__global__ void k_pad_keys(u64* keys, unsigned int n, unsigned int n_pad) {
-  unsigned int i = blockIdx.x * blockDim.x + threadIdx.x + n;
-  if (i < n_pad) keys[i] = ~0ull;
-}
-
-// ---- bitonic sort, ascending, length n_pad (power of two) -------------------------------
-constexpr int BT = 1024;            // threads per block
-constexpr int BTILE = 4 * BT;       // elements per block-local tile (32 KB of smem): 4096 -> 21 global steps for 2^18 keys
-constexpr int BPAIRS = BTILE / (2 * BT);   // compare-exchange pairs per thread and step
-
-__device__ __forceinline__ void cmpx(u64& a, u64& b, bool up) {
-  if ((a > b) == up) { u64 t = a; a = b; b = t; }
-}
-
-// sort each BTILE tile completely (all stages k <= BTILE)
-__global__ void __launch_bounds__(BT) k_bitonic_local_sort(u64* __restrict__ keys) {
-  __shared__ u64 sh[BTILE];
-  const unsigned int base = blockIdx.x * BTILE;
-  for (int e = threadIdx.x; e < BTILE; e += BT) sh[e] = keys[base + e];
-  __syncthreads();
-  for (unsigned int k = 2; k <= BTILE; k <<= 1) {
-    for (unsigned int j = k >> 1; j > 0; j >>= 1) {
-#pragma unroll
-      for (int q = 0; q < BPAIRS; ++q) {
-        const unsigned int t = threadIdx.x + q * BT;
-        const unsigned int i = 2 * t - (t & (j - 1));       // lower index of the pair
-        const bool up = (((base + i) & k) == 0);
-        cmpx(sh[i], sh[i + j], up);
-      }
-      __syncthreads();
-    }
-  }
-  for (int e = threadIdx.x; e < BTILE; e += BT) keys[base + e] = sh[e];
-}
-// one global compare-exchange step (j >= BTILE)
-__global__ void k_bitonic_global_step(u64* __restrict__ keys, unsigned int k, unsigned int j, unsigned int n_half) {
-  const unsigned int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_half) return;
-  const unsigned int i = 2 * t - (t & (j - 1));
-  const bool up = ((i & k) == 0);
-  u64 a = keys[i], b = keys[i + j];
-  if ((a > b) == up) { keys[i] = b; keys[i + j] = a; }
-}
-// finish stage k inside tiles: steps j = BTILE/2 .. 1
-__global__ void __launch_bounds__(BT) k_bitonic_local_merge(u64* __restrict__ keys, unsigned int k) {
-  __shared__ u64 sh[BTILE];
-  const unsigned int base = blockIdx.x * BTILE;
-  for (int e = threadIdx.x; e < BTILE; e += BT) sh[e] = keys[base + e];
-  __syncthreads();
-  for (unsigned int j = BTILE >> 1; j > 0; j >>= 1) {
-#pragma unroll
-    for (int q = 0; q < BPAIRS; ++q) {
-      const unsigned int t = threadIdx.x + q * BT;
-      const unsigned int i = 2 * t - (t & (j - 1));
-      const bool up = (((base + i) & k) == 0);
-      cmpx(sh[i], sh[i + j], up);
-    }
-    __syncthreads();
-  }
-  for (int e = threadIdx.x; e < BTILE; e += BT) keys[base + e] = sh[e];
 }
 
 __global__ void k_emit_sorted(const u64* __restrict__ keys, unsigned int n, const float* __restrict__ prob,
@@ -156,7 +96,7 @@ extern "C" int sdb_threshold_sort(const float* d_prob, int ndim, const int* shap
   *h_count = 0;
   if (npix == 0 || capacity <= 0) return 0;
   // keys buffer sized to the next power of two of capacity
-  unsigned int cap_pad = BTILE; while (cap_pad < (unsigned int)capacity) cap_pad <<= 1;
+  const unsigned int cap_pad = sdb::bitonic::padded_length((unsigned int)capacity);
   sdb::DevBuf b_keys, b_count;
   SDB_CUDA(b_keys.alloc((size_t)cap_pad * sizeof(u64), st));
   SDB_CUDA(b_count.alloc(sizeof(unsigned int), st));
@@ -169,14 +109,7 @@ extern "C" int sdb_threshold_sort(const float* d_prob, int ndim, const int* shap
   if (n > (unsigned int)capacity) { sdb::set_error("threshold_sort: candidate capacity exceeded"); return 1; }
   *h_count = (int)n;
   if (n == 0) return 0;
-  unsigned int n_pad = BTILE; while (n_pad < n) n_pad <<= 1;
-  if (n_pad > n) SDB_LAUNCH(k_pad_keys, cdiv(n_pad - n, 256), 256, 0, st, b_keys.as<u64>(), n, n_pad);
-  SDB_LAUNCH(k_bitonic_local_sort, n_pad / BTILE, BT, 0, st, b_keys.as<u64>());
-  for (unsigned int k = 2 * BTILE; k <= n_pad; k <<= 1) {
-    for (unsigned int j = k >> 1; j >= (unsigned int)BTILE; j >>= 1)
-      SDB_LAUNCH(k_bitonic_global_step, cdiv(n_pad / 2, 256), 256, 0, st, b_keys.as<u64>(), k, j, n_pad / 2);
-    SDB_LAUNCH(k_bitonic_local_merge, n_pad / BTILE, BT, 0, st, b_keys.as<u64>(), k);
-  }
+  if (sdb::bitonic::sort(b_keys.as<u64>(), n, sdb::bitonic::padded_length(n), st)) return 1;
   SDB_LAUNCH(k_emit_sorted, cdiv(n, 256), 256, 0, st, b_keys.as<u64>(), n, d_prob, d_sorted_index, d_sorted_prob);
   return 0;
 }

@@ -3,6 +3,8 @@ integer bookkeeping used by StarDist3D._instances_from_prediction (model3d.py:64
 predict_instances_big (base.py:959)."""
 import numpy as np
 
+from .utils import _raise
+
 
 def relabel_sequential(label_field, offset=1):
     """Relabel arbitrary labels to {`offset`, ... `offset` + number_of_labels}.
@@ -56,9 +58,76 @@ def relabel_sequential_device(label_field, offset=1, max_label=None):
     return label_field, fwd[:int(max_label) + 1], int(cnt.value)
 
 
+
+
+def label_overlap_device(a, b, capacity=1 << 16):
+    """Sparse label-overlap table of two device int32 label maps of the same shape (sdb_label_overlap): every distinct pair
+    (a[i], b[i]), background 0 included, sorted by (a, b).  Returns (pairs [m, 2] int32, counts [m] int64), device tensors.
+    `capacity`: first guess of the number of pairs; when it is too small the call is repeated once with the bound the
+    kernel reports.  Negative labels raise ValueError.  No CPU fallback: raises without the CUDA library."""
+    import ctypes, torch
+    from . import _lib as L
+    lib = L.require_cuda()
+    for t in (a, b):
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()):
+            raise ValueError("label_overlap_device expects contiguous CUDA int32 tensors")
+    if a.shape != b.shape:
+        raise ValueError("x and y must have the same shape")
+    n = a.numel()
+    cap = max(1, min(int(capacity), max(n, 1)))
+    for attempt in range(2):
+        pairs = torch.empty((cap, 2), dtype=torch.int32, device=a.device)
+        counts = torch.empty(cap, dtype=torch.int64, device=a.device)
+        m = ctypes.c_longlong(0)
+        rc = lib.sdb_label_overlap(L.ptr(a), L.ptr(b), n, L.ptr(pairs), L.ptr(counts), cap, ctypes.byref(m), L.stream_ptr())
+        if rc != 0:
+            if 'negative' in L.load().sdb_last_error().decode('utf-8', 'replace'):
+                raise ValueError("label maps must be arrays of non-negative integers.")
+            L.check(rc)
+        if m.value <= cap:
+            return pairs[:m.value], counts[:m.value]
+        cap = int(m.value)
+    raise L.StarDistB200Error("label_overlap: %d pairs do not fit the reported bound %d" % (m.value, cap))
+
+
 # ---------------------------------------------------------------------------------------------------------
-# Detection metrics (stardist/matching.py:109-232).  Host-side evaluation helper: pairs ground-truth and predicted
-# objects by an optimal assignment on the IoU (or IoT / IoP) matrix and counts tp / fp / fn at a threshold.
+# Detection metrics (stardist/matching.py:13-314).  Host-side evaluation: pairs ground-truth and predicted objects by an
+# optimal assignment on the IoU (or IoT / IoP) matrix and counts tp / fp / fn at one or several thresholds.
+MATCHING_CRITERIA = ('iou', 'iot', 'iop')
+_DATASET_KEYS = frozenset(('fp', 'tp', 'fn', 'precision', 'recall', 'accuracy', 'f1', 'criterion', 'thresh', 'n_true', 'n_pred',
+                           'mean_true_score', 'mean_matched_score', 'panoptic_quality'))
+
+
+def label_are_sequential(y):
+    """True if y has only the labels 1..max (and 0)"""
+    labels = np.unique(y)
+    return (set(labels) - {0}) == set(range(1, 1 + labels.max()))
+
+
+def _check_label_array(y, name=None, check_sequential=False):
+    err = ValueError("{label} must be an array of {integers}.".format(
+        label='labels' if name is None else name, integers=('sequential ' if check_sequential else '') + 'non-negative integers'))
+    if not (isinstance(y, np.ndarray) and np.issubdtype(y.dtype, np.integer)):
+        raise err
+    if len(y) == 0:
+        return True
+    if check_sequential:
+        label_are_sequential(y) or _raise(err)
+    else:
+        y.min() >= 0 or _raise(err)
+    return True
+
+
+def label_overlap(x, y, check=True):
+    """overlap[i, j] = number of pixels with label i in x and j in y, shape (1 + x.max(), 1 + y.max()), dtype np.uint
+    (stardist/matching.py:38-52).  With check, both must be arrays of sequential non-negative integers of one shape."""
+    if check:
+        _check_label_array(x, 'x', True)
+        _check_label_array(y, 'y', True)
+        x.shape == y.shape or _raise(ValueError("x and y must have the same shape"))
+    return _overlap_matrix(x, y).astype(np.uint)
+
+
 def _overlap_matrix(a, b):
     """counts[i, j] = number of pixels with label i in a and j in b (labels already sequential, 0 = background)"""
     na, nb = int(a.max()) + 1, int(b.max()) + 1
@@ -86,37 +155,117 @@ def _criterion_scores(overlap, criterion):
     raise ValueError("Matching criterion '%s' not supported." % criterion)
 
 
-def matching(y_true, y_pred, thresh=0.5, criterion='iou'):
-    """Matching(criterion, thresh, fp, tp, fn, precision, recall, accuracy, f1, n_true, n_pred, mean_true_score,
-    mean_matched_score, panoptic_quality) between two label images (stardist/matching.py:109-232)."""
+def matching_from_overlap(overlap, thresh=0.5, criterion='iou', report_matches=False, map_rev_true=None, map_rev_pred=None):
+    """The metrics of `matching` from the overlap matrix of two sequentially labelled images (row / column 0 = background):
+    one Matching for a scalar `thresh`, a tuple of them for a sequence (stardist/matching.py:155-230).  `map_rev_true` /
+    `map_rev_pred` map sequential ids back to the original ones for `report_matches` (default: identity)."""
     from collections import namedtuple
     from scipy.optimize import linear_sum_assignment
+    criterion in MATCHING_CRITERIA or _raise(ValueError("Matching criterion '%s' not supported." % criterion))
+    if thresh is None:
+        thresh = 0
+    single = np.isscalar(thresh)
+    threshs = (float(thresh),) if single else tuple(map(float, thresh))
+    scores = _criterion_scores(overlap, criterion)[1:, 1:]
+    n_true, n_pred = scores.shape
+    n_matched = min(n_true, n_pred)
+    rev_t = (lambda i: int(i)) if map_rev_true is None else (lambda i: int(map_rev_true[i]))
+    rev_p = (lambda j: int(j)) if map_rev_pred is None else (lambda j: int(map_rev_pred[j]))
+
+    def _single(thr):
+        tp, sum_matched = 0, 0.0
+        if n_matched > 0:
+            # maximise the number of pairs above the threshold, ties broken by the summed score (:185-190)
+            costs = -(scores >= thr).astype(float) - scores / (2 * n_matched)
+            ti, pi = linear_sum_assignment(costs)
+            ok = scores[ti, pi] >= thr
+            tp = np.count_nonzero(ok)                      # numpy integer scalar, as in the reference: float32 / np.int64 -> float64 below
+            sum_matched = np.sum(scores[ti, pi][ok])       # stays float32 like the reference's (matching.py:190): the means below are float32 quotients
+        fp, fn = n_pred - tp, n_true - tp
+        div = lambda a, b: (a / b) if np.abs(b) > 1e-10 else 0.0       # _safe_divide on scalars (matching.py:55-58)
+        # scalar types follow the reference's expressions (matching.py:180-196) so that the float results are the same numbers:
+        # sum (float32) / n_true (int) stays float32, / tp (numpy int) and / (tp + fp/2 + fn/2) are float64 quotients
+        fields = dict(criterion=criterion, thresh=thr, fp=fp, tp=tp, fn=fn,
+                      precision=(tp / (tp + fp) if tp > 0 else 0), recall=(tp / (tp + fn) if tp > 0 else 0),
+                      accuracy=(tp / (tp + fp + fn) if tp > 0 else 0), f1=((2 * tp) / (2 * tp + fp + fn) if tp > 0 else 0),
+                      n_true=n_true, n_pred=n_pred, mean_true_score=div(sum_matched, n_true),
+                      mean_matched_score=div(sum_matched, tp), panoptic_quality=div(sum_matched, tp + fp / 2 + fn / 2))
+        if bool(report_matches):
+            if n_matched > 0:                              # matching.py:208-219: every assigned pair, also those below thr
+                fields.update(matched_pairs=tuple((rev_t(i), rev_p(j)) for i, j in zip(1 + ti, 1 + pi)),
+                              matched_scores=tuple(scores[ti, pi]), matched_tps=tuple(map(int, np.flatnonzero(ok))))
+            else:
+                fields.update(matched_pairs=(), matched_scores=(), matched_tps=())
+        return namedtuple('Matching', fields.keys())(*fields.values())
+
+    return _single(threshs[0]) if single else tuple(map(_single, threshs))
+
+
+def matching(y_true, y_pred, thresh=0.5, criterion='iou', report_matches=False):
+    """Matching(criterion, thresh, fp, tp, fn, precision, recall, accuracy, f1, n_true, n_pred, mean_true_score,
+    mean_matched_score, panoptic_quality) between two label images (stardist/matching.py:109-232).  `thresh` may be a
+    sequence: then a tuple with one Matching per value.  report_matches adds matched_pairs (original ids), matched_scores
+    and matched_tps."""
     for name, y in (('y_true', y_true), ('y_pred', y_pred)):
         if not (isinstance(y, np.ndarray) and np.issubdtype(y.dtype, np.integer) and (y.size == 0 or y.min() >= 0)):
             raise ValueError("%s must be an array of non-negative integers." % name)
     if y_true.shape != y_pred.shape:
         raise ValueError("y_true and y_pred have different shapes")
-    thr = 0.0 if thresh is None else float(thresh)
-    yt = relabel_sequential(y_true)[0]
-    yp = relabel_sequential(y_pred)[0]
-    scores = _criterion_scores(_overlap_matrix(yt, yp), criterion)[1:, 1:]
-    n_true, n_pred = scores.shape
-    n_matched = min(n_true, n_pred)
-    tp, sum_matched = 0, 0.0
-    if n_matched > 0:
-        # maximise the number of pairs above the threshold, ties broken by the summed score (:185-190)
-        costs = -(scores >= thr).astype(float) - scores / (2 * n_matched)
-        ti, pi = linear_sum_assignment(costs)
-        ok = scores[ti, pi] >= thr
-        tp = np.count_nonzero(ok)                      # numpy integer scalar, as in the reference: float32 / np.int64 -> float64 below
-        sum_matched = np.sum(scores[ti, pi][ok])       # stays float32 like the reference's (matching.py:190): the means below are float32 quotients
-    fp, fn = n_pred - tp, n_true - tp
-    div = lambda a, b: (a / b) if np.abs(b) > 1e-10 else 0.0       # _safe_divide on scalars (matching.py:55-58)
-    # scalar types follow the reference's expressions (matching.py:180-196) so that the float results are the same numbers:
-    # sum (float32) / n_true (int) stays float32, / tp (numpy int) and / (tp + fp/2 + fn/2) are float64 quotients
-    fields = dict(criterion=criterion, thresh=thr, fp=fp, tp=tp, fn=fn,
-                  precision=(tp / (tp + fp) if tp > 0 else 0), recall=(tp / (tp + fn) if tp > 0 else 0),
-                  accuracy=(tp / (tp + fp + fn) if tp > 0 else 0), f1=((2 * tp) / (2 * tp + fp + fn) if tp > 0 else 0),
-                  n_true=n_true, n_pred=n_pred, mean_true_score=div(sum_matched, n_true),
-                  mean_matched_score=div(sum_matched, tp), panoptic_quality=div(sum_matched, tp + fp / 2 + fn / 2))
-    return namedtuple('Matching', fields.keys())(*fields.values())
+    criterion in MATCHING_CRITERIA or _raise(ValueError("Matching criterion '%s' not supported." % criterion))
+    yt, _, rev_t = relabel_sequential(y_true)
+    yp, _, rev_p = relabel_sequential(y_pred)
+    return matching_from_overlap(_overlap_matrix(yt, yp), thresh, criterion, report_matches, rev_t, rev_p)
+
+
+def accumulate_matching(stats_all, thresh, criterion='iou', by_image=False):
+    """DatasetMatching per threshold from per-image results (stardist/matching.py:270-314): stats_all holds, per image, the
+    tuple of Matching results for the thresholds `thresh` (a sequence).  Counts are summed; with by_image the ratios are
+    averaged over images, otherwise recomputed from the summed counts (mean_true_score accumulates as v * n_true)."""
+    from collections import namedtuple
+    n_images = len(stats_all)
+    accumulate = [{} for _ in thresh]
+    for stats in stats_all:
+        for acc, s in zip(accumulate, stats):
+            for k, v in s._asdict().items():
+                if k == 'mean_true_score' and not bool(by_image):
+                    acc[k] = acc.setdefault(k, 0) + v * s.n_true          # -> "sum_matched_score"
+                else:
+                    try:
+                        acc[k] = acc.setdefault(k, 0) + v
+                    except TypeError:
+                        pass
+    div = lambda a, b: (a / b) if np.abs(b) > 1e-10 else 0.0
+    for thr, acc in zip(thresh, accumulate):
+        set(acc.keys()) == _DATASET_KEYS or _raise(ValueError("unexpected keys"))
+        acc['criterion'] = criterion
+        acc['thresh'] = thr
+        acc['by_image'] = bool(by_image)
+        if bool(by_image):
+            for k in ('precision', 'recall', 'accuracy', 'f1', 'mean_true_score', 'mean_matched_score', 'panoptic_quality'):
+                acc[k] /= n_images
+        else:
+            tp, fp, fn, n_true = acc['tp'], acc['fp'], acc['fn'], acc['n_true']
+            sum_matched_score = acc['mean_true_score']
+            acc.update(precision=(tp / (tp + fp) if tp > 0 else 0), recall=(tp / (tp + fn) if tp > 0 else 0),
+                       accuracy=(tp / (tp + fp + fn) if tp > 0 else 0), f1=((2 * tp) / (2 * tp + fp + fn) if tp > 0 else 0),
+                       mean_true_score=div(sum_matched_score, n_true), mean_matched_score=div(sum_matched_score, tp),
+                       panoptic_quality=div(sum_matched_score, tp + fp / 2 + fn / 2))
+    return tuple(namedtuple('DatasetMatching', acc.keys())(*acc.values()) for acc in accumulate)
+
+
+def matching_dataset(y_true, y_pred, thresh=0.5, criterion='iou', by_image=False, show_progress=True, parallel=False):
+    """matching metrics for lists of images, see `matching` (stardist/matching.py:234-240).  show_progress and parallel are
+    accepted for compatibility; the images are evaluated in order."""
+    len(y_true) == len(y_pred) or _raise(ValueError("y_true and y_pred must have the same length."))
+    return matching_dataset_lazy(tuple(zip(y_true, y_pred)), thresh=thresh, criterion=criterion, by_image=by_image,
+                                 show_progress=show_progress, parallel=parallel)
+
+
+def matching_dataset_lazy(y_gen, thresh=0.5, criterion='iou', by_image=False, show_progress=True, parallel=False):
+    """matching_dataset over an iterable of (y_true, y_pred) pairs (stardist/matching.py:244-314): one DatasetMatching for a
+    scalar thresh, a tuple for a sequence."""
+    single = np.isscalar(thresh)
+    threshs = (thresh,) if single else tuple(thresh)
+    stats_all = tuple(matching(y_t, y_p, thresh=threshs, criterion=criterion, report_matches=False) for y_t, y_p in y_gen)
+    acc = accumulate_matching(stats_all, threshs, criterion=criterion, by_image=by_image)
+    return acc[0] if single else acc

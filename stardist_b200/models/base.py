@@ -4,8 +4,9 @@ Mirrors the prediction half of stardist/models/base.py:
   _predict_setup (:371-443), _predict_generator/predict (:446-529), _predict_sparse_generator/
   predict_sparse (:541-642), _predict_instances_generator/predict_instances (:645-790),
   predict_instances_big (:838-983), thresholds handling (:230-252), _compute_receptive_field
-  (:1068-1098), _axes_tile_overlap (:1101-1111), StarDistPadAndCropResizer (:1162-1211).
-Training, threshold optimisation and export are out of scope (DESIGN.md).
+  (:1068-1098), _axes_tile_overlap (:1101-1111), StarDistPadAndCropResizer (:1162-1211),
+  optimize_thresholds (:986-1043), _guess_n_tiles (:1046-1055).
+Training and export are out of scope (DESIGN.md).
 
 Differences by design: the network, thresholding, sort, NMS and label painting all run as CUDA
 kernels on tensors that stay in HBM; only the final labels / polygons are copied to the host.
@@ -468,17 +469,21 @@ class StarDistBase:
     # ------------------------------------------------------------------ predict (dense)
     def predict(self, img, axes=None, normalizer=None, n_tiles=None, show_tile_progress=True, **predict_kwargs):
         """Dense prediction: returns (prob, dist) numpy arrays (base.py:446-529)."""
+        return tuple(m.cpu().numpy() for m in self._predict_device(img, axes=axes, normalizer=normalizer, n_tiles=n_tiles))
+
+    def _predict_device(self, img, axes=None, normalizer=None, n_tiles=None):
+        """predict() with the cropped maps left in HBM: (prob, dist[, prob_class]) contiguous device tensors"""
         L.require_cuda()
         x, axes, axes_net, axes_net_div_by, _permute_axes, resizer, n_tiles, grid, grid_dict, channel = \
             self._predict_setup(img, axes, normalizer, n_tiles)
         prob_d, dist_d = self.predict_direct_device(self._to_device(x), n_tiles)
         sp_axes = axes_net.replace('C', '')
         crop = resizer.crop_slices(sp_axes, tuple(prob_d.shape))
-        prob = prob_d[crop].contiguous().cpu().numpy()
+        prob = prob_d[crop].contiguous()
         dist = dist_d[crop + (slice(None),)].contiguous()
-        dist = torch.clamp_min(dist, 1e-3).cpu().numpy()   # np.maximum(1e-3, dist), base.py:517
+        dist = torch.clamp_min(dist, 1e-3)                  # np.maximum(1e-3, dist), base.py:517
         if self._is_multiclass():                           # (prob, dist, prob_class), base.py:476-477,524-527
-            return prob, dist, self._last_class[crop + (slice(None),)].contiguous().cpu().numpy()
+            return prob, dist, self._last_class[crop + (slice(None),)].contiguous()
         return prob, dist
 
     # ------------------------------------------------------------------ predict_sparse
@@ -513,6 +518,19 @@ class StarDistBase:
         if sparse_store is None:
             prob_d, dist_d = self.predict_direct_device(x_dev, n_tiles)
         self._mark('net_end')
+        cand = self._candidates_from_maps(prob_d, dist_d, bounds, np.float32(prob_thresh), b=b, sparse_store=sparse_store)
+        self._mark('cand_end')
+        if self._is_multiclass():                           # prob_class[inds] of the candidates, base.py:595-614
+            pc = self._last_class
+            cand['prob_class'] = pc.reshape(-1, pc.shape[-1]).index_select(0, cand['index'].long())
+        return cand
+
+    def _candidates_from_maps(self, prob_d, dist_d, bounds, prob_thresh, b=2, sparse_store=None):
+        """device prob [...] / dist [..., R] maps (or the sparse candidate store) -> candidates with prob > prob_thresh
+        (float32) outside the border b and inside bounds (un-padded extent, image pixels): dict of device tensors prob[n],
+        dist[n, R], points_f32[n, nd] (index * grid), index[n] (flat map index), sorted by score (csrc/candidates.cu)."""
+        lib = L.require_cuda()
+        grid = tuple(self.config.grid)
         nd = self.config.n_dim
         R = self.config.n_rays
         shape = tuple(int(s) for s in prob_d.shape)
@@ -529,7 +547,7 @@ class StarDistBase:
         import ctypes
         cnt = ctypes.c_int(0)
         L.check(lib.sdb_threshold_sort(L.ptr(prob_d), nd, L.iarr(shape), L.iarr(valid), L.iarr([s[0] for s in bs]),
-                                      L.iarr([s[1] for s in bs]), float(np.float32(prob_thresh)), L.ptr(sidx), L.ptr(sprob),
+                                      L.iarr([s[1] for s in bs]), float(prob_thresh), L.ptr(sidx), L.ptr(sprob),
                                       npix, ctypes.byref(cnt), L.stream_ptr()))
         n = int(cnt.value)
         self._last_n_cand = n
@@ -542,12 +560,7 @@ class StarDistBase:
         else:
             L.check(lib.sdb_gather_candidates(L.ptr(dist_d), L.ptr(sidx), n, R, nd, L.iarr(shape), L.iarr(grid),
                                              L.ptr(dist_s), L.ptr(pts_f), L.stream_ptr()))
-        self._mark('cand_end')
-        cand = dict(prob=sprob, dist=dist_s, points_f32=pts_f, n=n)
-        if self._is_multiclass():                           # prob_class[inds] of the candidates, base.py:595-614
-            pc = self._last_class
-            cand['prob_class'] = pc.reshape(-1, pc.shape[-1]).index_select(0, sidx.long())
-        return cand
+        return dict(prob=sprob, dist=dist_s, points_f32=pts_f, n=n, index=sidx)
 
     def _use_sparse_forward(self, x_dev, n_tiles):
         """slab-wise sparse forward (UNetDevice3DTC.forward_candidates): STARDIST_B200_SPARSE_FORWARD = 1 / 0 / auto
@@ -779,6 +792,59 @@ class StarDistBase:
             if k in out:
                 out[k] = block.translate_coordinates(out[k], axes=axes_out)
         return tile, out, len(ind)
+
+    # ------------------------------------------------------------------ threshold optimisation
+    def optimize_thresholds(self, X_val, Y_val, nms_threshs=[0.3, 0.4, 0.5], iou_threshs=[0.3, 0.5, 0.7], predict_kwargs=None,
+                            optimize_kwargs=None, save_to_json=True):
+        """Optimize the two thresholds (probability, NMS overlap) of predict_instances (base.py:986-1043).
+
+        For every value of nms_threshs, utils.optimize_threshold finds the prob_thresh with the best matching performance on
+        (X_val, Y_val), averaged over iou_threshs; the best pair becomes self.thresholds and, with save_to_json and a model
+        folder, <logdir>/thresholds.json.  X_val must be normalized.  predict_kwargs go to predict (default n_tiles:
+        _guess_n_tiles); optimize_kwargs to utils.optimize_threshold.  The predicted maps stay in HBM for the search."""
+        from ..utils import optimize_threshold
+        import sys
+        if predict_kwargs is None:
+            predict_kwargs = {}
+        if optimize_kwargs is None:
+            optimize_kwargs = {}
+
+        def _predict_kwargs(x):
+            if 'n_tiles' in predict_kwargs:
+                return predict_kwargs
+            return {**predict_kwargs, 'n_tiles': self._guess_n_tiles(x), 'show_tile_progress': False}
+
+        def _predict(x, axes=None, normalizer=None, n_tiles=None, show_tile_progress=True, **kw):
+            # predict()'s signature (other keywords are accepted and ignored, as there); only (prob, dist) of a multi-class model
+            return self._predict_device(x, axes=axes, normalizer=normalizer, n_tiles=n_tiles)[:2]
+        Yhat_val = [_predict(x, **_predict_kwargs(x)) for x in X_val]
+        opt_prob_thresh, opt_measure, opt_nms_thresh = None, -np.inf, None
+        for _opt_nms_thresh in nms_threshs:
+            _opt_prob_thresh, _opt_measure = optimize_threshold(Y_val, Yhat_val, model=self, nms_thresh=_opt_nms_thresh,
+                                                                iou_threshs=iou_threshs, **optimize_kwargs)
+            if _opt_measure > opt_measure:
+                opt_prob_thresh, opt_measure, opt_nms_thresh = _opt_prob_thresh, _opt_measure, _opt_nms_thresh
+        opt_threshs = dict(prob=opt_prob_thresh, nms=opt_nms_thresh)
+        self.thresholds = opt_threshs
+        print(end='', file=sys.stderr, flush=True)
+        print("Using optimized values: prob_thresh={prob:g}, nms_thresh={nms:g}.".format(prob=self.thresholds.prob, nms=self.thresholds.nms))
+        if save_to_json and self.logdir is not None:
+            print("Saving to 'thresholds.json'.")
+            with open(self.logdir / 'thresholds.json', 'w') as f:
+                json.dump({k: float(v) for k, v in opt_threshs.items()}, f)
+        return opt_threshs
+
+    def _guess_n_tiles(self, img):
+        """tiles per image axis so that a tile holds about one training batch of patches (base.py:1046-1055)"""
+        axes = self._normalize_axes(img, axes=None)
+        shape = list(img.shape)
+        if 'C' in axes:
+            del shape[axes_dict(axes)['C']]
+        b = self.config.train_batch_size ** (1.0 / self.config.n_dim)
+        n_tiles = [int(np.ceil(s / (p * b))) for s, p in zip(shape, self.config.train_patch_size)]
+        if 'C' in axes:
+            n_tiles.insert(axes_dict(axes)['C'], 1)
+        return tuple(n_tiles)
 
     # ------------------------------------------------------------------ misc
     def _compute_receptive_field(self, img_size=None):

@@ -95,3 +95,39 @@ def normalize_mi_ma(x, mi, ma, clip=False, eps=1e-20, dtype=np.float32):
 
 def _is_floatarray(x):
     return isinstance(x.dtype.type(0), np.floating)
+
+
+def optimize_threshold(Y, Yhat, model, nms_thresh, measure='accuracy', iou_threshs=[0.3, 0.5, 0.7], bracket=None, tol=1e-2, maxiter=20, verbose=1):
+    """Tune prob_thresh for a fixed nms_thresh to maximise `measure` of matching_dataset averaged over iou_threshs
+    (stardist/utils.py:271-307): a golden-section search over prob_thresh in `bracket` (default: half the largest prob to
+    the largest).  Y: ground-truth label images, Yhat: (prob, dist) per image as `model.predict` returns them (numpy arrays;
+    device tensors are used in place).  Returns (prob_thresh, value).
+
+    Same search and values as the reference; each value comes from the threshold engine (stardist_b200/optimize.py), which
+    runs the NMS, label painting and overlap table once per image and restricts them to each probe."""
+    import datetime
+    from scipy.optimize import minimize_scalar
+    from . import optimize as E
+    np.isscalar(nms_thresh) or _raise(ValueError("nms_thresh must be a scalar"))
+    iou_threshs = [iou_threshs] if np.isscalar(iou_threshs) else iou_threshs
+    values = dict()
+
+    if bracket is None:
+        max_prob = max([(np.float32(prob.max().item()) if hasattr(prob, 'is_cuda') else np.max(prob)) for prob, dist in Yhat])
+        bracket = max_prob / 2, max_prob
+    tables = [E.image_tables(model, y, prob, dist, nms_thresh, t_floor=min(bracket)) for y, (prob, dist) in zip(Y, Yhat)]
+
+    def fn(thr):
+        prob_thresh = np.clip(thr, *bracket)
+        value = values.get(prob_thresh)
+        if value is None:
+            stats = E.dataset_matching(tables, prob_thresh, iou_threshs)
+            values[prob_thresh] = value = np.mean([s._asdict()[measure] for s in stats])
+        if verbose > 1:
+            print("{now}   thresh: {prob_thresh:f}   {measure}: {value:f}".format(
+                now=datetime.datetime.now().strftime('%H:%M:%S'), prob_thresh=prob_thresh, measure=measure, value=value), flush=True)
+        return -value
+
+    opt = minimize_scalar(fn, method='golden', bracket=bracket, tol=tol, options={'maxiter': maxiter})
+    verbose > 1 and print('\n', opt, flush=True)
+    return opt.x, -opt.fun
