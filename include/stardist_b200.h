@@ -155,6 +155,37 @@ int sdb_relabel_sequential(int* d_labels, long long n, int max_label, int offset
 int sdb_label_overlap(const int* d_a, const int* d_b, long long n, int* d_pairs, long long* d_counts,
                       long long capacity, long long* h_n_pairs, sdb_stream_t stream);
 
+/* star distances (stardist2d.cpp:55-125 c_star_dist, stardist3d.cpp:245-345 c_star_dist3d), bit-identical to the reference.
+ * d_labels: label map [H, W] / [D, H, W], uint16 (label_bytes 2) or int32 (label_bytes 4); labels are compared by their low
+ * 16 bits (the reference's astype(np.uint16)).  h_dirs: HOST float32 table [2][n_rays] = [dy | dx] (dy = cosf(phi_k),
+ * dx = sinf(phi_k), phi_k = float(k) * float(2 pi / n_rays), libm's single-precision functions) or h_rays [3][n_rays] =
+ * [dz | dy | dx] (Rays.vertices as float32).  Dense mode (d_points NULL): d_out float32 [Ho, Wo(, ...), n_rays] with
+ * Ho = (H - 1) / grid_y + 1 etc.  Point mode: d_points int32 [n_points][2 or 3] indices into that subsampled grid, d_out
+ * float32 [n_points][n_rays].  A ray set whose walk cannot be bounded for the shape is an error (sdb_star_dist_walk_bound). */
+int sdb_star_dist_2d(const void* d_labels, int label_bytes, int H, int W, int grid_y, int grid_x, int n_rays,
+                     const float* h_dirs, const int* d_points, long long n_points, float* d_out, sdb_stream_t stream);
+int sdb_star_dist_3d(const void* d_labels, int label_bytes, int D, int H, int W, int grid_z, int grid_y, int grid_x,
+                     int n_rays, const float* h_rays, const int* d_points, long long n_points, float* d_out,
+                     sdb_stream_t stream);
+/* host-only check of a direction table ([ndim][n_rays], as above) for an image of the given shape: every ray needs a
+ * component of magnitude >= max(2^-8, 2 ulp(max extent + 1 + max component)).  On success *h_cap = a step count after
+ * which every walk has left the image (the kernels' loop cap); otherwise an error and a message. */
+int sdb_star_dist_walk_bound(const float* h_dirs, int ndim, int n_rays, const int* shape, long long* h_cap);
+/* host-pointer versions with the reference's semantics: src uint16, dst float32 dense; void, on failure dst is zeroed and
+ * sdb_last_error() holds the message (cleared on success) */
+void _LIB_star_dist_2d(const unsigned short* src, int H, int W, int n_rays, int grid_y, int grid_x, const float* dirs,
+                       float* dst);
+void _LIB_star_dist_3d(const unsigned short* src, int D, int H, int W, int n_rays, int grid_z, int grid_y, int grid_x,
+                       const float* rays, float* dst);
+
+/* per-label statistics of a sequential int32 label map (values in [0, n_labels], e.g. after sdb_relabel_sequential):
+ * for label l >= 1, index l - 1: d_count[n_labels] pixel count, d_sum[n_labels][ndim] coordinate sums, d_bbox_min /
+ * d_bbox_max [n_labels][ndim] smallest / largest coordinate (inclusive), axes in array order.  What regionprops gives
+ * relabel_image_stardist (centroid = sum / count) and calculate_extents (bbox).  shape is a host int[ndim].  Negative
+ * labels or labels above n_labels are an error.  Synchronises the stream once. */
+int sdb_region_stats(const int* d_labels, int ndim, const int* shape, int n_labels, long long* d_count, long long* d_sum,
+                     int* d_bbox_min, int* d_bbox_max, sdb_stream_t stream);
+
 /* 3D NMS on device arrays (see _LIB_non_maximum_suppression_sparse); d_keep is uint8[n_polys]. */
 int sdb_nms3d(const float* d_dist, const float* d_points, const float* d_verts, const int* d_faces,
               int n_polys, int n_rays, int n_faces, float threshold, int use_bbox, int use_kdtree,

@@ -9,8 +9,9 @@ __version__ = "0.1.0"
 from .nms import (non_maximum_suppression, non_maximum_suppression_sparse, non_maximum_suppression_inds,
                   non_maximum_suppression_3d, non_maximum_suppression_3d_sparse, non_maximum_suppression_3d_inds)
 from .geometry import (ray_angles, dist_to_coord, polygons_to_label, polygons_to_label_coord,
-                       polyhedron_to_label, dist_to_coord3D)
+                       polyhedron_to_label, dist_to_coord3D, star_dist, star_dist3D, relabel_image_stardist,
+                       relabel_image_stardist3D)
 from .rays3d import Rays_GoldenSpiral, Rays_Explicit, Rays_Cartesian, Rays_SubDivide, Rays_Tetra, Rays_Octo, rays_from_json
 from .matching import relabel_sequential
 from .models import Config2D, StarDist2D, Config3D, StarDist3D
-from .utils import normalize
+from .utils import normalize, calculate_extents

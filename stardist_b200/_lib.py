@@ -88,6 +88,18 @@ def _declare(lib):
     lib.sdb_relabel_sequential.restype = c_int
     lib.sdb_label_overlap.argtypes = [P, P, c_longlong, P, P, c_longlong, POINTER(c_longlong), P]
     lib.sdb_label_overlap.restype = c_int
+    lib.sdb_star_dist_2d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_longlong, P, P]
+    lib.sdb_star_dist_2d.restype = c_int
+    lib.sdb_star_dist_3d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_longlong, P, P]
+    lib.sdb_star_dist_3d.restype = c_int
+    lib.sdb_star_dist_walk_bound.argtypes = [P, c_int, c_int, P, POINTER(c_longlong)]
+    lib.sdb_star_dist_walk_bound.restype = c_int
+    lib._LIB_star_dist_2d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, P, P]
+    lib._LIB_star_dist_2d.restype = None
+    lib._LIB_star_dist_3d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P]
+    lib._LIB_star_dist_3d.restype = None
+    lib.sdb_region_stats.argtypes = [P, c_int, P, c_int, P, P, P, P, P]
+    lib.sdb_region_stats.restype = c_int
     lib.sdb_nms3d.argtypes = [P, P, P, P, c_int, c_int, c_int, c_float, c_int, c_int, c_int, P, P]
     lib.sdb_unet_layer_count.argtypes = [P]
     lib.sdb_unet_layer_count.restype = c_int

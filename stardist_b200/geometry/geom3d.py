@@ -3,6 +3,8 @@
 Mirrors stardist/geometry/geom3d.py: polyhedron_to_label (:100-198), dist_to_coord3D (:261-275).
 """
 import numpy as np
+from ..utils import _normalize_grid
+from .distances import star_dist3D_device, label_map_to_device, centroids_device, check_points_in, output_shape
 
 
 RENDER_MODES = ("full", "kernel", "hull", "bbox", "debug")      # index = render_mode of the C entry point
@@ -63,3 +65,66 @@ def dist_to_coord3D(dist, points, rays_vertices):
                 points.shape[-1] == 3, rays_vertices.shape[-1] == 3, dist.shape[-1] == len(rays_vertices))):
         raise ValueError(f"Wrong shapes! dist -> (m,n) points -> (m,3) rays_vertices -> (m,)")
     return points[:, np.newaxis] + dist[..., np.newaxis] * rays_vertices
+
+
+def star_dist3D(lbl, rays, grid=(1, 1, 1), mode='cpp'):
+    """lbl assumbed to be a label image with integer values that encode object ids. id 0 denotes background.
+
+    Star distances float32 [(D-1)//gz+1, (H-1)//gy+1, (W-1)//gx+1, len(rays)] along rays.vertices
+    (stardist/geometry/geom3d.py:17-24, 87-97), bit-identical to the reference's C++.  Modes 'cpp' and 'opencl' both run
+    the CUDA kernel with the C++ semantics; there is no 'python' mode (no CPU fallback)."""
+    import torch
+    from .. import _lib as L
+    grid = _normalize_grid(grid, 3)
+    if mode == 'python':
+        raise NotImplementedError("star_dist3D: mode 'python' has no CPU implementation here; use 'cpp'")
+    if mode not in ('cpp', 'opencl'):
+        raise ValueError("Unknown mode %s" % mode)
+    L.require_cuda()
+    lbl = np.asarray(lbl).astype(np.uint16, copy=False)
+    if lbl.ndim != 3:
+        raise ValueError("star_dist3D: label image must be 3-dimensional")
+    d = torch.from_numpy(np.ascontiguousarray(lbl)).to("cuda")
+    return star_dist3D_device(d, rays, grid).cpu().numpy()
+
+
+def relabel_image_stardist3D(lbl, rays, verbose=False, **kwargs):
+    """relabel each label region in `lbl` with its star representation (stardist/geometry/geom3d.py:201-217): the
+    polyhedron of the star distances (at least 1e-3) at each region's centroid, painted by polyhedron_to_label with the
+    region labels.  Centroids, distances and painting stay on the device; `kwargs` (grid) as in star_dist3D, including the
+    reference's indexing of the subsampled map with full-resolution centroids (IndexError where numpy raises)."""
+    import torch
+    from .. import _lib as L
+    from ..matching import _check_label_array
+    _check_label_array(lbl, "lbl")
+    if not lbl.ndim == 3:
+        raise ValueError("lbl image should be 3 dimensional")
+    mode = kwargs.pop('mode', 'cpp')
+    grid = _normalize_grid(kwargs.pop('grid', (1, 1, 1)), 3)
+    if kwargs:
+        raise TypeError("unexpected keyword arguments %s" % sorted(kwargs))
+    if mode == 'python':
+        raise NotImplementedError("star_dist3D: mode 'python' has no CPU implementation here; use 'cpp'")
+    lib = L.require_cuda()
+    seq, n, labels = label_map_to_device(lbl)
+    d_lbl = torch.from_numpy(np.ascontiguousarray(lbl.astype(np.uint16, copy=False))).to("cuda")
+    points = centroids_device(seq, n) if n > 0 else torch.zeros((0, 3), dtype=torch.int32, device="cuda")
+    check_points_in(points, output_shape(lbl.shape, grid))
+    dist = star_dist3D_device(d_lbl, rays, grid, points=points)
+    if n == 0:
+        verbose and print("warning: empty list of points (returning background-only image)")
+        return np.zeros(lbl.shape, np.uint16)
+    dist = torch.clamp_min(dist, 1e-3)
+    # the region labels in ascending order (regionprops), painted as polyhedron_to_label paints equal scores: last first
+    flip = torch.arange(n - 1, -1, -1, device="cuda")
+    dist, pts, labels = dist[flip].contiguous(), points[flip].to(torch.float32).contiguous(), labels[flip].contiguous()
+    verts = torch.from_numpy(np.ascontiguousarray(rays.vertices, np.float32)).to("cuda")
+    faces = torch.from_numpy(np.ascontiguousarray(rays.faces, np.int32)).to("cuda")
+    nz, ny, nx = lbl.shape
+    out = torch.empty((nz, ny, nx), dtype=torch.int32, device="cuda")
+    if verbose:
+        print("+++++++++++++++ polyhedra to label (GPU) +++++++++++++++ \nn_polys = %d n_rays = %d n_faces = %d nz,ny,nx = %d %d %d"
+              % (n, len(rays), len(rays.faces), nz, ny, nx))
+    L.check(lib.sdb_polyhedron_to_label(L.ptr(dist), L.ptr(pts), L.ptr(verts), L.ptr(faces), n, len(rays), len(rays.faces),
+                                        L.ptr(labels), nz, ny, nx, RENDER_MODES.index("full"), 0, 0, L.ptr(out), L.stream_ptr()))
+    return out.cpu().numpy()

@@ -3,6 +3,8 @@
 c_non_max_suppression_inds(dist f32[n,R] C-contig, points f32[n,2], use_kdtree:int, use_bbox:int,
                            verbose:int, thresh:f32) -> bool[n]         ("O!O!iiif", stardist2d.cpp:396)
 Inputs must be sorted by descending score (as stardist/nms.py:186-227 guarantees).
+c_star_dist(src uint16[H,W], n_rays:int, grid_y:int, grid_x:int) -> float32[(H-1)//grid_y+1, (W-1)//grid_x+1, n_rays]
+                                                                     ("O!iii", stardist2d.cpp:55-125)
 """
 import numpy as np
 from .. import _lib as L
@@ -23,3 +25,24 @@ def c_non_max_suppression_inds(dist, points, use_kdtree, use_bbox, verbose, thre
         L.check(lib._LIB_non_maximum_suppression_2d(L.ptr(dist), L.ptr(points), n, R, float(thresh),
                                                    int(use_bbox), int(use_kdtree), int(verbose), L.ptr(result)))
     return result
+
+
+def c_star_dist(src, n_rays, grid_y, grid_x):
+    from ..geometry.distances import direction_table_2d, walk_bound, output_shape
+    if not isinstance(src, np.ndarray):
+        raise TypeError("src must be a numpy array")
+    if src.dtype != np.uint16 or src.ndim != 2:
+        raise TypeError("src must be a 2-dimensional uint16 array")
+    n_rays, gy, gx = int(n_rays), int(grid_y), int(grid_x)
+    if n_rays < 1 or gy < 1 or gx < 1:
+        raise ValueError("n_rays, grid_y and grid_x must be >= 1")
+    lib = L.require_cuda()
+    dirs = np.ascontiguousarray(direction_table_2d(n_rays))
+    walk_bound(dirs, src.shape)
+    src = np.ascontiguousarray(src)
+    dst = np.empty(output_shape(src.shape, (gy, gx)) + (n_rays,), np.float32)
+    lib._LIB_star_dist_2d(L.ptr(src), src.shape[0], src.shape[1], n_rays, gy, gx, L.ptr(dirs), L.ptr(dst))
+    msg = lib.sdb_last_error()
+    if msg:
+        raise L.StarDistB200Error(msg.decode("utf-8", "replace"))
+    return dst

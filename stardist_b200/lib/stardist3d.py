@@ -7,6 +7,9 @@ c_non_max_suppression_inds(dist f32[n,R], points f32[n,3], verts f32[R,3], faces
 c_polyhedron_to_label(dist, points, verts, faces, labels i32[n], render_mode:int, verbose:int,
                       use_overlap_label:int, overlap_label:int, (nz,ny,nx)) -> int32[nz,ny,nx]
                                                         ("O!O!O!O!O!iiii(iii)", stardist3d.cpp:93)
+c_star_dist3d(src uint16[D,H,W], dz, dy, dx float32[n_rays], n_rays:int, grid_z:int, grid_y:int, grid_x:int)
+                      -> float32[(D-1)//grid_z+1, (H-1)//grid_y+1, (W-1)//grid_x+1, n_rays]
+                                                        ("O!O!O!O!iiii", stardist3d.cpp:245-345)
 Inputs must be sorted by descending score.  Backed by the reference-signature C ABI
 _LIB_non_maximum_suppression_sparse / _LIB_polyhedron_to_label of libstardist_b200.so.
 """
@@ -69,3 +72,22 @@ def c_polyhedron_to_label(dist, points, verts, faces, labels, render_mode, verbo
       int(render_mode), int(verbose), int(use_overlap_label), int(overlap_label), L.ptr(result))
     _raise_on_error(lib)
     return result
+
+
+def c_star_dist3d(src, dz, dy, dx, n_rays, grid_z, grid_y, grid_x):
+    from ..geometry.distances import walk_bound, output_shape
+    src = _chk(src, np.uint16, 3, "src")
+    n_rays = int(n_rays)
+    comps = [_chk(a, np.float32, 1, name) for a, name in ((dz, "dz"), (dy, "dy"), (dx, "dx"))]
+    if n_rays < 1 or any(len(a) < n_rays for a in comps):
+        raise ValueError("n_rays must be >= 1 and dz, dy, dx must hold n_rays values each")
+    grid = tuple(int(g) for g in (grid_z, grid_y, grid_x))
+    if min(grid) < 1:
+        raise ValueError("grid values must be >= 1")
+    lib = L.require_cuda()
+    rays = np.ascontiguousarray(np.stack([a[:n_rays] for a in comps]))
+    walk_bound(rays, src.shape)
+    dst = np.empty(output_shape(src.shape, grid) + (n_rays,), np.float32)
+    lib._LIB_star_dist_3d(L.ptr(src), *src.shape, n_rays, *grid, L.ptr(rays), L.ptr(dst))
+    _raise_on_error(lib)
+    return dst

@@ -131,3 +131,23 @@ def optimize_threshold(Y, Yhat, model, nms_thresh, measure='accuracy', iou_thres
     opt = minimize_scalar(fn, method='golden', bracket=bracket, tol=tol, options={'maxiter': maxiter})
     verbose > 1 and print('\n', opt, flush=True)
     return opt.x, -opt.fun
+
+
+def calculate_extents(lbl, func=np.median):
+    """ Aggregate bounding box sizes of objects in label images. (stardist/utils.py:180-193)
+
+    The bounding boxes come from sdb_region_stats on the device, one per label in ascending label order, as regionprops
+    lists them."""
+    if (isinstance(lbl, np.ndarray) and lbl.ndim == 4) or (not isinstance(lbl, np.ndarray) and isinstance(lbl, Iterable)):
+        return func(np.stack([calculate_extents(_lbl, func) for _lbl in lbl], axis=0), axis=0)
+
+    n = lbl.ndim
+    n in (2, 3) or _raise(ValueError("label image should be 2- or 3-dimensional (or pass a list of these)"))
+
+    from .geometry.distances import label_map_to_device, region_stats_device
+    seq, n_labels, _ = label_map_to_device(lbl)
+    if n_labels == 0:
+        return np.zeros(n)
+    _, _, bmin, bmax = region_stats_device(seq, n_labels)
+    extents = (bmax.to(dtype=bmin.dtype) - bmin + 1).cpu().numpy().astype(np.int64)
+    return func(extents, axis=0)
