@@ -186,6 +186,25 @@ void _LIB_star_dist_3d(const unsigned short* src, int D, int H, int W, int n_ray
 int sdb_region_stats(const int* d_labels, int ndim, const int* shape, int n_labels, long long* d_count, long long* d_sum,
                      int* d_bbox_min, int* d_bbox_max, sdb_stream_t stream);
 
+/* training targets (stardist/utils.py:98-153, _edt_prob_scipy and fill_label_holes), bit-identical to the reference.
+ * d_labels: sequential int32 label map (values 0..n_labels, e.g. after sdb_relabel_sequential; negative labels mapped to 0
+ * first), shape a host int[ndim], ndim 2 or 3, every extent <= 65535, at most 2^31 - 1 pixels.
+ * sdb_edt_prob: d_prob float32 = float(sqrt(d2) / (sqrt(max of d2 over the label) + 1e-10)), d2 = squared distance to the
+ * nearest pixel of another label, sum_a ((q_a - p_a) * s_a)^2 in float64 in axis order; h_sampling: HOST double[ndim]
+ * (NULL = 1); black_border: positions just outside the image count as another label (the reference's constant-image rule).
+ * sdb_fill_label_holes: d_out int32 = the largest label whose pixels or holes contain the pixel, 0 elsewhere; holes are
+ * connected under generate_binary_structure(ndim, connectivity), connectivity in [1, ndim].  Uses sdb_region_stats and
+ * synchronises the stream once (box sizes). */
+int sdb_edt_prob(const int* d_labels, int ndim, const int* shape, int n_labels, const double* h_sampling, int black_border,
+                 float* d_prob, sdb_stream_t stream);
+int sdb_fill_label_holes(const int* d_labels, int ndim, const int* shape, int n_labels, int connectivity, int* d_out,
+                         sdb_stream_t stream);
+/* host-pointer versions on any int32 label map (negative labels are never an object; relabelling, the constant-image rule and
+ * the mapping back to the original labels happen inside): void, on failure the result is zeroed and sdb_last_error() holds
+ * the message (cleared on success) */
+void _LIB_edt_prob(const int* lbl, int ndim, const int* shape, const double* sampling, float* prob);
+void _LIB_fill_label_holes(const int* lbl, int ndim, const int* shape, int connectivity, int* out);
+
 /* 3D NMS on device arrays (see _LIB_non_maximum_suppression_sparse); d_keep is uint8[n_polys]. */
 int sdb_nms3d(const float* d_dist, const float* d_points, const float* d_verts, const int* d_faces,
               int n_polys, int n_rays, int n_faces, float threshold, int use_bbox, int use_kdtree,

@@ -100,6 +100,14 @@ def _declare(lib):
     lib._LIB_star_dist_3d.restype = None
     lib.sdb_region_stats.argtypes = [P, c_int, P, c_int, P, P, P, P, P]
     lib.sdb_region_stats.restype = c_int
+    lib.sdb_edt_prob.argtypes = [P, c_int, P, c_int, P, c_int, P, P]
+    lib.sdb_edt_prob.restype = c_int
+    lib.sdb_fill_label_holes.argtypes = [P, c_int, P, c_int, c_int, P, P]
+    lib.sdb_fill_label_holes.restype = c_int
+    lib._LIB_edt_prob.argtypes = [P, c_int, P, P, P]
+    lib._LIB_edt_prob.restype = None
+    lib._LIB_fill_label_holes.argtypes = [P, c_int, P, c_int, P]
+    lib._LIB_fill_label_holes.restype = None
     lib.sdb_nms3d.argtypes = [P, P, P, P, c_int, c_int, c_int, c_float, c_int, c_int, c_int, P, P]
     lib.sdb_unet_layer_count.argtypes = [P]
     lib.sdb_unet_layer_count.restype = c_int

@@ -133,6 +133,24 @@ def optimize_threshold(Y, Yhat, model, nms_thresh, measure='accuracy', iou_thres
     return opt.x, -opt.fun
 
 
+def edt_prob(lbl_img, anisotropy=None):
+    """Perform EDT on each labeled object and normalize. (stardist/utils.py:71-125)
+
+    Equal to the reference's scipy variant bit for bit: one multi-label exact distance transform of the whole map on the
+    device (stardist_b200/labelprep.py, csrc/labelprep.cu) instead of one scipy call per object."""
+    from .labelprep import edt_prob as _edt_prob
+    return _edt_prob(lbl_img, anisotropy=anisotropy)
+
+
+def fill_label_holes(lbl_img, **kwargs):
+    """Fill small holes in label image. (stardist/utils.py:137-153)
+
+    All labels at once on the device (stardist_b200/labelprep.py); kwargs as binary_fill_holes takes them, with `structure`
+    one of generate_binary_structure(ndim, c)."""
+    from .labelprep import fill_label_holes as _fill_label_holes
+    return _fill_label_holes(lbl_img, **kwargs)
+
+
 def calculate_extents(lbl, func=np.median):
     """ Aggregate bounding box sizes of objects in label images. (stardist/utils.py:180-193)
 
