@@ -178,6 +178,12 @@ void _LIB_star_dist_2d(const unsigned short* src, int H, int W, int n_rays, int 
 void _LIB_star_dist_3d(const unsigned short* src, int D, int H, int W, int n_rays, int grid_z, int grid_y, int grid_x,
                        const float* rays, float* dst);
 
+/* batched dense star distances for training batches: d_labels int32 [batch][shape...] (maps laid end to end, each walked on
+ * its own), d_out float32 [batch][Ho][Wo](...) with n_rays values at the start of every out_stride floats (out_stride
+ * n_rays + 1 leaves a channel free: the dist_and_mask layout).  Same walk and table as sdb_star_dist_2d / _3d. */
+int sdb_star_dist_batch(const int* d_labels, int ndim, int batch, const int* shape, const int* grid, int n_rays,
+                        const float* h_dirs, int out_stride, float* d_out, sdb_stream_t stream);
+
 /* per-label statistics of a sequential int32 label map (values in [0, n_labels], e.g. after sdb_relabel_sequential):
  * for label l >= 1, index l - 1: d_count[n_labels] pixel count, d_sum[n_labels][ndim] coordinate sums, d_bbox_min /
  * d_bbox_max [n_labels][ndim] smallest / largest coordinate (inclusive), axes in array order.  What regionprops gives
@@ -199,6 +205,35 @@ int sdb_edt_prob(const int* d_labels, int ndim, const int* shape, int n_labels, 
                  float* d_prob, sdb_stream_t stream);
 int sdb_fill_label_holes(const int* d_labels, int ndim, const int* shape, int n_labels, int connectivity, int* d_out,
                          sdb_stream_t stream);
+/* edt_prob of `batch` maps of `shape` laid end to end (no pass crosses an item; the constant-image rule is decided per item
+ * from its label minimum and maximum, written to d_item_minmax int32 [batch][2]).  Labels are distinct across items, values
+ * 0..n_labels.  Output at the grid positions (Do = (D - 1) / grid + 1 ...): d_prob float32 [batch][Do..] (-1 where d_neg,
+ * uint8 [batch][Do..] or NULL, is set) and, when d_dist_and_mask is not NULL, the unmasked value at d_dist_and_mask[o *
+ * dm_stride].  Does not synchronise. */
+int sdb_edt_prob_batch(const int* d_labels, int ndim, int batch, const int* shape, int n_labels, const double* h_sampling,
+                       const int* grid, const unsigned char* d_neg, int* d_item_minmax, float* d_prob, float* d_dist_and_mask,
+                       int dm_stride, sdb_stream_t stream);
+
+/* training batches (stardist/models/base.py:129-225, model2d.py:29-120, model3d.py:30-127, sample_patches.py).
+ * sdb_fg_valid_index: d_mask uint8 [shape] = maximum_filter(labels, filter_size, mode='constant') > 0 and d_prefix int64
+ * [rows + 1] = the prefix count of set positions over the rows of the box [p//2, s-p+p//2] (rows: every axis but the last,
+ * C order); *h_n_valid (host) = d_prefix[rows].  Synchronises the stream once.
+ * sdb_sample_select: positions (int32 [batch][3], 2-D: 0 first) of the drawn ranks of the items d_items (int64
+ * [batch][10], see traindata.cu).  sdb_train_gather: patches at those positions -> d_x float32 [batch][patch][n_channels],
+ * d_y_clamped int32 max(label, 0) (the label itself when clamp is 0), d_y_slots int32 (per-item sequential labels + the item's slot offset), and at the grid
+ * positions d_neg uint8 (label < 0) and, if not NULL, d_y_slots_grid; d_flags[0] |= 1 where a slot with class -2 (no class
+ * given) occurs.  sdb_class_map: prob_class float32 [batch][out_shape][n_classes + 1] (mask_to_categorical of the slots'
+ * classes d_class_table, -1 = None, then scipy's order-0 zoom with the source indices d_zoom_index int32 [sum out_shape],
+ * then -1 where d_neg). */
+int sdb_fg_valid_index(const int* d_labels, int ndim, const int* shape, const int* filter_size, const int* patch_size,
+                       unsigned char* d_mask, long long* d_prefix, long long* h_n_valid, sdb_stream_t stream);
+int sdb_sample_select(const long long* d_items, int ndim, int batch, const int* patch_size, int* d_pos, sdb_stream_t stream);
+int sdb_train_gather(const long long* d_items, const int* d_pos, int ndim, int batch, const int* patch_size, int n_channels,
+                     const int* grid, const int* d_class_table, float* d_x, int* d_y_clamped, int* d_y_slots,
+                     int* d_y_slots_grid, unsigned char* d_neg, int* d_flags, int clamp, sdb_stream_t stream);
+int sdb_class_map(const int* d_y_slots, int ndim, int batch, const int* patch_size, const int* d_zoom_index,
+                  const int* out_shape, const int* d_class_table, int n_classes, const unsigned char* d_neg, float* d_out,
+                  sdb_stream_t stream);
 /* host-pointer versions on any int32 label map (negative labels are never an object; relabelling, the constant-image rule and
  * the mapping back to the original labels happen inside): void, on failure the result is zeroed and sdb_last_error() holds
  * the message (cleared on success) */

@@ -102,6 +102,18 @@ def _declare(lib):
     lib.sdb_region_stats.restype = c_int
     lib.sdb_edt_prob.argtypes = [P, c_int, P, c_int, P, c_int, P, P]
     lib.sdb_edt_prob.restype = c_int
+    lib.sdb_star_dist_batch.argtypes = [P, c_int, c_int, P, P, c_int, P, c_int, P, P]
+    lib.sdb_star_dist_batch.restype = c_int
+    lib.sdb_edt_prob_batch.argtypes = [P, c_int, c_int, P, c_int, P, P, P, P, P, P, c_int, P]
+    lib.sdb_edt_prob_batch.restype = c_int
+    lib.sdb_fg_valid_index.argtypes = [P, c_int, P, P, P, P, P, POINTER(c_longlong), P]
+    lib.sdb_fg_valid_index.restype = c_int
+    lib.sdb_sample_select.argtypes = [P, c_int, c_int, P, P, P]
+    lib.sdb_sample_select.restype = c_int
+    lib.sdb_train_gather.argtypes = [P, P, c_int, c_int, P, c_int, P, P, P, P, P, P, P, P, c_int, P]
+    lib.sdb_train_gather.restype = c_int
+    lib.sdb_class_map.argtypes = [P, c_int, c_int, P, P, P, P, c_int, P, P, P]
+    lib.sdb_class_map.restype = c_int
     lib.sdb_fill_label_holes.argtypes = [P, c_int, P, c_int, c_int, P, P]
     lib.sdb_fill_label_holes.restype = c_int
     lib._LIB_edt_prob.argtypes = [P, c_int, P, P, P]

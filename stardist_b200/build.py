@@ -11,7 +11,7 @@ COMMON = ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler",
 UNITS = [
     ("runtime.cu", False), ("candidates.cu", True), ("nms2d.cu", True), ("nms2d_nv32.cu", True),
     ("nms2d_nv128.cu", True), ("label2d.cu", True), ("label3d.cu", True), ("blocks.cu", True), ("prep.cu", True), ("nms3d.cu", True), ("unet_simt.cu", False), ("unet_tc.cu", False), ("unet_exec.cu", False), ("overlap.cu", False),
-    ("stardist.cu", True), ("labelprep.cu", True),
+    ("stardist.cu", True), ("labelprep.cu", True), ("traindata.cu", True),
 ]
 
 def _deps(src):

@@ -15,7 +15,9 @@
 // (Felzenszwalb & Huttenlocher), built with an exact cross-multiplied test.  Every pass carries the arg-min offset
 // vector instead of a distance, and the last pass recomputes d2 from it in scipy's order and rounding, so integer and
 // dyadic sampling are exact (all products and sums stay below 2^53 for extents <= 65535).  This unit is built with
-// -fmad=false so no product is contracted into an FMA.
+// -fmad=false so no product is contracted into an FMA.  sdb_edt_prob_batch runs the same passes over training patches laid
+// end to end: no pass runs along the batch (an object at a patch edge sees only its own patch, as the reference's per-patch
+// call does), labels are distinct across items, and the constant-image rule is decided per item.
 //
 // fill_label_holes (reference: stardist/utils.py:137-153).  For label i, holes are the pixels with a label != i inside
 // i's bounding box grown by one pixel on the sides that do not touch the image border, which cannot reach the boundary
@@ -48,10 +50,15 @@ template <int NB, bool FINAL>
 __global__ void __launch_bounds__(EDT_THREADS) k_edt_pass(const int* __restrict__ lbl, int len, long long inner, long long n_lines,
                                                           long long N, const int* __restrict__ in, int* __restrict__ out,
                                                           double* __restrict__ d2, unsigned long long* __restrict__ lmax, Samp sp,
-                                                          int black, int* __restrict__ sv, double* __restrict__ sf) {
+                                                          int black, const int* __restrict__ item_minmax, long long item_lines,
+                                                          int* __restrict__ sv, double* __restrict__ sf) {
   const long long l = (long long)blockIdx.x * EDT_THREADS + threadIdx.x;
   if (l >= n_lines) return;
   const long long o = l / inner, base = o * len * inner + (l - o * inner);
+  if (item_minmax) {                        // batch: the constant-image rule per item (its label minimum equals its maximum > 0)
+    const long long it = l / item_lines;
+    black = item_minmax[2 * it] == item_minmax[2 * it + 1] && item_minmax[2 * it + 1] > 0;
+  }
   const double s = sp.s[0], w = s * s;
   int* v = sv + l;
   double* f = sf + l;
@@ -264,6 +271,51 @@ int check_shape(const char* what, int ndim, const int* shape, int dims[3], long 
 
 int grid_for(long long work, int threads) { return (int)std::max<long long>(1, std::min<long long>(cdiv(work, threads), 132 * 32)); }
 
+// the passes of the transform over `batch` maps of `shape` laid end to end (no pass runs along the batch): d2 of every pixel
+// and the per-label maximum lmax[n_labels] (labels distinct across items).  item_minmax (device [batch][2], or NULL for the
+// scalar black_border) gives each item's constant-image rule.
+int edt_passes(const int* d_labels, int ndim, const int* shape, int batch, long long N, const double* s, int black_border,
+               const int* item_minmax, int n_labels, double* D2, unsigned long long* M, cudaStream_t st) {
+  long long stack = 0;                               // envelope entries of the largest pass: (len + 2) per line
+  for (int a = 0; a < ndim; ++a) stack = std::max(stack, (shape[a] + 2LL) * (N / shape[a]));
+  sdb::DevBuf offs_a, offs_b, sv, sf;
+  SDB_CUDA(offs_a.alloc((size_t)N * 4, st));
+  if (ndim == 3) SDB_CUDA(offs_b.alloc((size_t)N * 4 * 2, st));
+  SDB_CUDA(sv.alloc((size_t)stack * 4, st));
+  SDB_CUDA(sf.alloc((size_t)stack * 8, st));
+  SDB_CUDA(cudaMemsetAsync(M, 0, (size_t)n_labels * 8, st));
+  auto geom = [&](int a, int& len, long long& inner, long long& lines) {
+    len = shape[a];
+    inner = 1;
+    for (int b = a + 1; b < ndim; ++b) inner *= shape[b];
+    lines = N / len;
+  };
+  auto samp = [&](int a) { Samp p{{1.0, 1.0, 1.0}}; for (int b = a; b < ndim; ++b) p.s[b - a] = s[b]; return p; };
+  int len;
+  long long inner, lines;
+  int* A = offs_a.as<int>();
+  int* B = offs_b.as<int>();
+  int* SV = sv.as<int>();
+  double* SF = sf.as<double>();
+  const int* MM = item_minmax;
+  geom(ndim - 1, len, inner, lines);
+  SDB_LAUNCH((k_edt_pass<0, false>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, nullptr, A, nullptr,
+             nullptr, samp(ndim - 1), black_border, MM, lines / batch, SV, SF);
+  if (ndim == 2) {
+    geom(0, len, inner, lines);
+    SDB_LAUNCH((k_edt_pass<1, true>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, A, nullptr, D2, M,
+               samp(0), black_border, MM, lines / batch, SV, SF);
+  } else {
+    geom(1, len, inner, lines);
+    SDB_LAUNCH((k_edt_pass<1, false>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, A, B, nullptr,
+               nullptr, samp(1), black_border, MM, lines / batch, SV, SF);
+    geom(0, len, inner, lines);
+    SDB_LAUNCH((k_edt_pass<2, true>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, B, nullptr, D2, M,
+               samp(0), black_border, MM, lines / batch, SV, SF);
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" int sdb_edt_prob(const int* d_labels, int ndim, const int* shape, int n_labels, const double* h_sampling, int black_border,
@@ -280,47 +332,95 @@ extern "C" int sdb_edt_prob(const int* d_labels, int ndim, const int* shape, int
   }
   if (N == 0) return 0;
   if (n_labels == 0) { SDB_CUDA(cudaMemsetAsync(d_prob, 0, (size_t)N * 4, st)); return 0; }
-  long long stack = 0;                               // envelope entries of the largest pass: (len + 2) per line
-  for (int a = 0; a < ndim; ++a) stack = std::max(stack, (shape[a] + 2LL) * (N / shape[a]));
-  sdb::DevBuf offs_a, offs_b, d2, lmax, sv, sf;
-  SDB_CUDA(offs_a.alloc((size_t)N * 4, st));
-  if (ndim == 3) SDB_CUDA(offs_b.alloc((size_t)N * 4 * 2, st));
+  sdb::DevBuf d2, lmax;
   SDB_CUDA(d2.alloc((size_t)N * 8, st));
   SDB_CUDA(lmax.alloc((size_t)n_labels * 8, st));
-  SDB_CUDA(sv.alloc((size_t)stack * 4, st));
-  SDB_CUDA(sf.alloc((size_t)stack * 8, st));
-  SDB_CUDA(cudaMemsetAsync(lmax.p, 0, (size_t)n_labels * 8, st));
-  auto geom = [&](int a, int& len, long long& inner, long long& lines) {
-    len = shape[a];
-    inner = 1;
-    for (int b = a + 1; b < ndim; ++b) inner *= shape[b];
-    lines = N / len;
-  };
-  auto samp = [&](int a) { Samp p{{1.0, 1.0, 1.0}}; for (int b = a; b < ndim; ++b) p.s[b - a] = s[b]; return p; };
-  int len;
-  long long inner, lines;
-  int* A = offs_a.as<int>();
-  int* B = offs_b.as<int>();
   double* D2 = d2.as<double>();
   unsigned long long* M = lmax.as<unsigned long long>();
-  int* SV = sv.as<int>();
-  double* SF = sf.as<double>();
-  geom(ndim - 1, len, inner, lines);
-  SDB_LAUNCH((k_edt_pass<0, false>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, nullptr, A, nullptr,
-             nullptr, samp(ndim - 1), black_border, SV, SF);
-  if (ndim == 2) {
-    geom(0, len, inner, lines);
-    SDB_LAUNCH((k_edt_pass<1, true>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, A, nullptr, D2, M,
-               samp(0), black_border, SV, SF);
-  } else {
-    geom(1, len, inner, lines);
-    SDB_LAUNCH((k_edt_pass<1, false>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, A, B, nullptr,
-               nullptr, samp(1), black_border, SV, SF);
-    geom(0, len, inner, lines);
-    SDB_LAUNCH((k_edt_pass<2, true>), cdiv(lines, EDT_THREADS), EDT_THREADS, 0, st, d_labels, len, inner, lines, N, B, nullptr, D2, M,
-               samp(0), black_border, SV, SF);
-  }
+  if (edt_passes(d_labels, ndim, shape, 1, N, s, black_border, nullptr, n_labels, D2, M, st)) return 1;
   SDB_LAUNCH(k_edt_norm, grid_for(N, 256), 256, 0, st, d_labels, D2, M, N, d_prob);
+  return 0;
+}
+
+namespace {
+
+__global__ void k_minmax_init(int* __restrict__ mm, int batch) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < batch) { mm[2 * b] = INT_MAX; mm[2 * b + 1] = INT_MIN; }
+}
+
+// per-item label minimum and maximum; grid (blocks per item, batch)
+__global__ void k_item_minmax(const int* __restrict__ lbl, long long n_item, int* __restrict__ mm) {
+  const int b = blockIdx.y;
+  const int* l = lbl + (long long)b * n_item;
+  int lo = INT_MAX, hi = INT_MIN;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_item; i += (long long)gridDim.x * blockDim.x) {
+    const int v = __ldg(l + i);
+    lo = min(lo, v); hi = max(hi, v);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+  }
+  if ((threadIdx.x & 31) == 0) { atomicMin(mm + 2 * b, lo); atomicMax(mm + 2 * b + 1, hi); }
+}
+
+// normalisation at the grid positions of every item: prob[b, o] (-1 where neg[b, o]) and dam[(b, o) * dm_stride], the
+// unmasked value
+__global__ void k_edt_norm_grid(const int* __restrict__ lbl, const double* __restrict__ d2, const unsigned long long* __restrict__ lmax,
+                                int D, int H, int W, int gz, int gy, int gx, int Do, int Ho, int Wo, long long n_out,
+                                const unsigned char* __restrict__ neg, float* __restrict__ prob, float* __restrict__ dam, int dm_stride) {
+  for (long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x; o < n_out; o += (long long)gridDim.x * blockDim.x) {
+    const int k = (int)(o % Wo);
+    const long long t = o / Wo;
+    const int j = (int)(t % Ho);
+    const long long u = t / Ho;
+    const int i = (int)(u % Do);
+    const long long b = u / Do;
+    const long long src = ((b * D + (long long)i * gz) * H + (long long)j * gy) * W + (long long)k * gx;
+    const int L = __ldg(lbl + src);
+    float r = 0.f;
+    if (L > 0) {
+      const double m = __longlong_as_double((long long)__ldg(lmax + (L - 1)));
+      r = __double2float_rn(__ddiv_rn(__dsqrt_rn(d2[src]), __dadd_rn(__dsqrt_rn(m), 1e-10)));
+    }
+    prob[o] = (neg && neg[o]) ? -1.f : r;
+    if (dam) dam[o * dm_stride] = r;
+  }
+}
+
+}  // namespace
+
+extern "C" int sdb_edt_prob_batch(const int* d_labels, int ndim, int batch, const int* shape, int n_labels, const double* h_sampling,
+                                  const int* grid, const unsigned char* d_neg, int* d_item_minmax, float* d_prob, float* d_dist_and_mask,
+                                  int dm_stride, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  int dims[3];
+  long long n_item;
+  if (check_shape("edt_prob", ndim, shape, dims, &n_item)) return 1;
+  if (batch < 1 || n_labels < 0) { sdb::set_error("edt_prob: batch must be >= 1 and n_labels >= 0"); return 1; }
+  double s[3] = {1.0, 1.0, 1.0};
+  int g[3] = {1, 1, 1}, od[3] = {1, 1, 1};
+  for (int a = 0; a < ndim; ++a) {
+    if (h_sampling) s[a] = h_sampling[a];
+    if (!(s[a] > 0.0) || !std::isfinite(s[a])) { sdb::set_error("edt_prob: sampling must be positive and finite"); return 1; }
+    if (grid[a] < 1) { sdb::set_error("edt_prob: grid values must be >= 1"); return 1; }
+    g[3 - ndim + a] = grid[a];
+    od[3 - ndim + a] = (shape[a] - 1) / grid[a] + 1;
+  }
+  if (n_item == 0) return 0;
+  const long long N = n_item * batch;
+  SDB_LAUNCH(k_minmax_init, cdiv(batch, 128), 128, 0, st, d_item_minmax, batch);
+  SDB_LAUNCH(k_item_minmax, dim3((unsigned)std::min<long long>(cdiv(n_item, 256), 64), (unsigned)batch), 256, 0, st, d_labels, n_item,
+             d_item_minmax);
+  sdb::DevBuf d2, lmax;
+  SDB_CUDA(d2.alloc((size_t)N * 8, st));
+  SDB_CUDA(lmax.alloc((size_t)n_labels * 8, st));
+  if (edt_passes(d_labels, ndim, shape, batch, N, s, 0, d_item_minmax, n_labels, d2.as<double>(), lmax.as<unsigned long long>(), st))
+    return 1;
+  const long long n_out = (long long)batch * od[0] * od[1] * od[2];
+  SDB_LAUNCH(k_edt_norm_grid, grid_for(n_out, 256), 256, 0, st, d_labels, d2.as<double>(), lmax.as<unsigned long long>(), dims[0], dims[1],
+             dims[2], g[0], g[1], g[2], od[0], od[1], od[2], n_out, d_neg, d_prob, d_dist_and_mask, dm_stride);
   return 0;
 }
 

@@ -10,7 +10,8 @@
 // One warp per output pixel, lanes over the rays: a pixel's R floats are written as one coalesced run and a background
 // pixel exits uniformly per warp.  The walk is bounded: sdb_star_dist_walk_bound (host) rejects ray sets that could
 // stall for the given shape and returns the step count after which every walk has left the image; the kernels use it
-// as a hard cap (unreachable for accepted inputs; reaching it would write NaN).
+// as a hard cap (unreachable for accepted inputs; reaching it would write NaN).  sdb_star_dist_batch walks a batch of maps
+// laid end to end, each on its own, and writes every pixel's R floats at a stride (the dist_and_mask layout of training).
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -33,20 +34,23 @@ __device__ __forceinline__ unsigned short lbl16(const T* __restrict__ p, long lo
 template <typename T>
 __global__ void __launch_bounds__(SD_THREADS) k_star_dist_2d(const T* __restrict__ lbl, int H, int W, int gy, int gx, int Ho, int Wo,
                                                              const float* __restrict__ dirs, int R, const int* __restrict__ points,
-                                                             long long n_out, long long cap, float* __restrict__ out) {
+                                                             long long n_out, long long n_item, int ostride, long long cap,
+                                                             float* __restrict__ out) {
   const long long p = (long long)blockIdx.x * SD_WARPS + (threadIdx.x >> 5);
   if (p >= n_out) return;
   const int lane = threadIdx.x & 31;
-  float* o = out + p * R;
+  const long long b = p / n_item, q = p - b * n_item;       // batch item, output pixel within it
+  lbl += b * H * W;
+  float* o = out + p * ostride;
   int i, j;
   if (points) {
-    i = points[2 * p]; j = points[2 * p + 1];
+    i = points[2 * q]; j = points[2 * q + 1];
     if (i < 0 || i >= Ho || j < 0 || j >= Wo) {           // the callers validate; never read outside the map
       for (int k = lane; k < R; k += 32) o[k] = __int_as_float(0x7fc00000);
       return;
     }
   } else {
-    i = (int)(p / Wo); j = (int)(p - (long long)i * Wo);
+    i = (int)(q / Wo); j = (int)(q - (long long)i * Wo);
   }
   const int pi = i * gy, pj = j * gx;
   const unsigned short value = lbl16(lbl, (long long)pi * W + pj);
@@ -79,23 +83,25 @@ __global__ void __launch_bounds__(SD_THREADS) k_star_dist_2d(const T* __restrict
 template <typename T>
 __global__ void __launch_bounds__(SD_THREADS) k_star_dist_3d(const T* __restrict__ lbl, int D, int H, int W, int gz, int gy, int gx,
                                                              int Do, int Ho, int Wo, const float* __restrict__ rays, int R,
-                                                             const int* __restrict__ points, long long n_out, long long cap,
-                                                             float* __restrict__ out) {
+                                                             const int* __restrict__ points, long long n_out, long long n_item,
+                                                             int ostride, long long cap, float* __restrict__ out) {
   const long long p = (long long)blockIdx.x * SD_WARPS + (threadIdx.x >> 5);
   if (p >= n_out) return;
   const int lane = threadIdx.x & 31;
-  float* o = out + p * R;
+  const long long b = p / n_item, q = p - b * n_item;
+  lbl += b * D * H * W;
+  float* o = out + p * ostride;
   int i, j, l;
   if (points) {
-    i = points[3 * p]; j = points[3 * p + 1]; l = points[3 * p + 2];
+    i = points[3 * q]; j = points[3 * q + 1]; l = points[3 * q + 2];
     if (i < 0 || i >= Do || j < 0 || j >= Ho || l < 0 || l >= Wo) {
       for (int k = lane; k < R; k += 32) o[k] = __int_as_float(0x7fc00000);
       return;
     }
   } else {
     const long long plane = (long long)Ho * Wo;
-    i = (int)(p / plane);
-    const long long r = p - (long long)i * plane;
+    i = (int)(q / plane);
+    const long long r = q - (long long)i * plane;
     j = (int)(r / Wo); l = (int)(r - (long long)j * Wo);
   }
   const int pi = i * gz, pj = j * gy, pl = l * gx;
@@ -204,9 +210,14 @@ extern "C" int sdb_star_dist_walk_bound(const float* h_dirs, int ndim, int n_ray
 namespace {
 
 // shared by the 2-D and 3-D entry points: bound, table upload, launch
-int star_dist_launch(int ndim, const void* d_labels, int label_bytes, const int* shape, const int* grid, int n_rays,
-                     const float* h_dirs, const int* d_points, long long n_points, float* d_out, cudaStream_t st) {
+// batch maps of `shape` laid end to end (dense mode only for batch > 1); output pixel p of the whole batch is written at
+// d_out + p * ostride (ostride = n_rays for a plain [..., n_rays] map)
+int star_dist_launch(int ndim, const void* d_labels, int label_bytes, int batch, const int* shape, const int* grid, int n_rays,
+                     const float* h_dirs, const int* d_points, long long n_points, int ostride, float* d_out, cudaStream_t st) {
   if (label_bytes != 2 && label_bytes != 4) { sdb::set_error("star_dist: labels must be uint16 (2 bytes) or int32 (4 bytes)"); return 1; }
+  if (batch < 1 || (batch > 1 && d_points) || ostride < n_rays) {
+    sdb::set_error("star_dist: batch must be >= 1 (1 in point mode) and the output stride >= n_rays"); return 1;
+  }
   int oshape[3];
   for (int a = 0; a < ndim; ++a) {
     if (grid[a] < 1) { sdb::set_error("star_dist: grid values must be >= 1"); return 1; }
@@ -215,9 +226,10 @@ int star_dist_launch(int ndim, const void* d_labels, int label_bytes, const int*
   long long cap = 0;
   if (sdb_star_dist_walk_bound(h_dirs, ndim, n_rays, shape, &cap)) return 1;
   if (n_points < 0) { sdb::set_error("star_dist: n_points must be >= 0"); return 1; }
-  long long n_out = n_points;
-  if (!d_points) { n_out = 1; for (int a = 0; a < ndim; ++a) n_out *= oshape[a]; }
-  if (n_out == 0) return 0;
+  long long n_item = n_points;
+  if (!d_points) { n_item = 1; for (int a = 0; a < ndim; ++a) n_item *= oshape[a]; }
+  if (n_item == 0) return 0;
+  const long long n_out = n_item * batch;
   sdb::DevBuf d_dirs;
   SDB_CUDA(d_dirs.alloc((size_t)ndim * n_rays * sizeof(float), st));
   SDB_CUDA(cudaMemcpyAsync(d_dirs.p, h_dirs, (size_t)ndim * n_rays * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -226,19 +238,19 @@ int star_dist_launch(int ndim, const void* d_labels, int label_bytes, const int*
   if (ndim == 2) {
     if (label_bytes == 2)
       SDB_LAUNCH(k_star_dist_2d<unsigned short>, (int)blocks, SD_THREADS, 0, st, (const unsigned short*)d_labels, shape[0], shape[1],
-                 grid[0], grid[1], oshape[0], oshape[1], d_dirs.as<float>(), n_rays, d_points, n_out, cap, d_out);
+                 grid[0], grid[1], oshape[0], oshape[1], d_dirs.as<float>(), n_rays, d_points, n_out, n_item, ostride, cap, d_out);
     else
       SDB_LAUNCH(k_star_dist_2d<int>, (int)blocks, SD_THREADS, 0, st, (const int*)d_labels, shape[0], shape[1],
-                 grid[0], grid[1], oshape[0], oshape[1], d_dirs.as<float>(), n_rays, d_points, n_out, cap, d_out);
+                 grid[0], grid[1], oshape[0], oshape[1], d_dirs.as<float>(), n_rays, d_points, n_out, n_item, ostride, cap, d_out);
   } else {
     if (label_bytes == 2)
       SDB_LAUNCH(k_star_dist_3d<unsigned short>, (int)blocks, SD_THREADS, 0, st, (const unsigned short*)d_labels, shape[0], shape[1],
                  shape[2], grid[0], grid[1], grid[2], oshape[0], oshape[1], oshape[2], d_dirs.as<float>(), n_rays, d_points, n_out,
-                 cap, d_out);
+                 n_item, ostride, cap, d_out);
     else
       SDB_LAUNCH(k_star_dist_3d<int>, (int)blocks, SD_THREADS, 0, st, (const int*)d_labels, shape[0], shape[1],
                  shape[2], grid[0], grid[1], grid[2], oshape[0], oshape[1], oshape[2], d_dirs.as<float>(), n_rays, d_points, n_out,
-                 cap, d_out);
+                 n_item, ostride, cap, d_out);
   }
   return 0;
 }
@@ -255,7 +267,7 @@ void star_dist_host(int ndim, const unsigned short* src, const int* shape, const
     SDB_CUDA(d_src.alloc((size_t)n_in * 2, st));
     SDB_CUDA(d_dst.alloc((size_t)n_out * 4, st));
     SDB_CUDA(cudaMemcpyAsync(d_src.p, src, (size_t)n_in * 2, cudaMemcpyHostToDevice, st));
-    if (star_dist_launch(ndim, d_src.p, 2, shape, grid, n_rays, dirs, nullptr, 0, d_dst.as<float>(), st)) return 1;
+    if (star_dist_launch(ndim, d_src.p, 2, 1, shape, grid, n_rays, dirs, nullptr, 0, n_rays, d_dst.as<float>(), st)) return 1;
     SDB_CUDA(cudaMemcpyAsync(dst, d_dst.p, (size_t)n_out * 4, cudaMemcpyDeviceToHost, st));
     SDB_CUDA(cudaStreamSynchronize(st));
     return 0;
@@ -273,14 +285,20 @@ void star_dist_host(int ndim, const unsigned short* src, const int* shape, const
 extern "C" int sdb_star_dist_2d(const void* d_labels, int label_bytes, int H, int W, int grid_y, int grid_x, int n_rays,
                                 const float* h_dirs, const int* d_points, long long n_points, float* d_out, sdb_stream_t stream) {
   const int shape[2] = {H, W}, grid[2] = {grid_y, grid_x};
-  return star_dist_launch(2, d_labels, label_bytes, shape, grid, n_rays, h_dirs, d_points, n_points, d_out, (cudaStream_t)stream);
+  return star_dist_launch(2, d_labels, label_bytes, 1, shape, grid, n_rays, h_dirs, d_points, n_points, n_rays, d_out, (cudaStream_t)stream);
 }
 
 extern "C" int sdb_star_dist_3d(const void* d_labels, int label_bytes, int D, int H, int W, int grid_z, int grid_y, int grid_x,
                                 int n_rays, const float* h_rays, const int* d_points, long long n_points, float* d_out,
                                 sdb_stream_t stream) {
   const int shape[3] = {D, H, W}, grid[3] = {grid_z, grid_y, grid_x};
-  return star_dist_launch(3, d_labels, label_bytes, shape, grid, n_rays, h_rays, d_points, n_points, d_out, (cudaStream_t)stream);
+  return star_dist_launch(3, d_labels, label_bytes, 1, shape, grid, n_rays, h_rays, d_points, n_points, n_rays, d_out, (cudaStream_t)stream);
+}
+
+extern "C" int sdb_star_dist_batch(const int* d_labels, int ndim, int batch, const int* shape, const int* grid, int n_rays,
+                                   const float* h_dirs, int out_stride, float* d_out, sdb_stream_t stream) {
+  if (ndim != 2 && ndim != 3) { sdb::set_error("star_dist: ndim must be 2 or 3"); return 1; }
+  return star_dist_launch(ndim, d_labels, 4, batch, shape, grid, n_rays, h_dirs, nullptr, 0, out_stride, d_out, (cudaStream_t)stream);
 }
 
 extern "C" void _LIB_star_dist_2d(const unsigned short* src, int H, int W, int n_rays, int grid_y, int grid_x, const float* dirs,

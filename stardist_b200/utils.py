@@ -169,3 +169,14 @@ def calculate_extents(lbl, func=np.median):
     _, _, bmin, bmax = region_stats_device(seq, n_labels)
     extents = (bmax.to(dtype=bmin.dtype) - bmin + 1).cpu().numpy().astype(np.int64)
     return func(extents, axis=0)
+
+
+def grid_divisible_patch_size(patch_size, grid, warn=True):
+    # stardist/utils.py:397-403
+    import warnings
+    patch_size, grid = tuple(patch_size), tuple(grid)
+    assert len(patch_size) == len(grid)
+    patch_size_divisible = tuple(int(np.ceil(sh / g) * g) for sh, g in zip(patch_size, grid))
+    if patch_size != patch_size_divisible and warn:
+        warnings.warn(f"increasing patch_size from {patch_size} to {patch_size_divisible}, since it was not evenly divisible by grid {grid}")
+    return patch_size_divisible
