@@ -390,6 +390,40 @@ void sdb_unet_destroy(sdb_unet* net);
 int _LIB_unet_forward_2d(sdb_unet* net, const float* d_x, int h, int w, float* d_prob, float* d_dist, sdb_stream_t stream);
 int _LIB_unet_forward_3d(sdb_unet* net, const float* d_x, int d, int h, int w, float* d_prob, float* d_dist, sdb_stream_t stream);
 
+/* ---- training step of the U-Net (csrc/unet_train.cu): fp32 CUDA cores, fixed-order reductions, no float atomics ----
+ * Weight gradient of a 3^d (kz = 3 in 3-D, 1 in 2-D; kyx = 3) or 1^d (kz = kyx = 1) 'same' convolution over the whole batch:
+ * dw (k..., cin, cout) = sum_p x[p + tap] * dy[p], db = sum_p dy[p]; the input is [upsample(x_lo), skip] as in sdb_conv3_nd,
+ * dy has row stride ldy >= cout.  d_work holds sdb_conv_wgrad_workspace(n*d*h*w, taps, cin_skip + cin_lo, cout) floats. */
+long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin, int cout);
+int sdb_conv_wgrad_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                      int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
+                      long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
+/* wf (k..., cout, cin) = w (k..., cin, cout) flipped along every spatial axis: the input gradient of a stride-1 'same'
+ * convolution is sdb_conv3_nd of dy with wf, zero bias, no ReLU */
+int sdb_conv_flip_weights(const float* d_w, int taps, int cin, int cout, float* d_wf, sdb_stream_t stream);
+/* gradient of [upsample(x_lo), skip] -> d x_lo (block sums, the backward of nearest up-sampling) and d skip (overwritten) */
+int sdb_decoder_split(const float* d_dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy, int ux,
+                      float* d_dlo, float* d_dskip, sdb_stream_t stream);
+/* g *= (y > 0) in place, y the saved ReLU output */
+int sdb_relu_backward(float* d_g, const float* d_y, long long n, sdb_stream_t stream);
+/* gradient of sdb_maxpool_nd to the first maximum of each window (row-major); accumulate = 1 adds to d_gx */
+int sdb_maxpool_backward_nd(const float* d_x, const float* d_gy, int n, int d, int h, int w, int c, int pz, int py, int px,
+                            int accumulate, float* d_gx, sdb_stream_t stream);
+/* StarDist loss (DESIGN.md 4.2): prob = sigmoid output [npix], dist [npix][n_rays], targets prob_t [npix] and dist_and_mask
+ * [npix][n_rays + 1].  Writes stats (n_p, mean mask), out = (loss, prob_loss, dist_loss, n_p == 0) and, if d_dhead is not NULL,
+ * dhead [npix][n_rays + 1] = (dL/d prob logit, dL/d dist).  d_state (optional) = (t, n_skipped, skip) of the training step.
+ * d_work holds sdb_stardist_loss_workspace(npix) bytes. */
+long long sdb_stardist_loss_workspace(long long npix);
+int sdb_stardist_loss(const float* d_prob, const float* d_dist, const float* d_prob_t, const float* d_dam, long long npix,
+                      int n_rays, int mae, float lam, float w0, float w1, void* d_work, float* d_stats, float* d_dhead,
+                      float* d_out, int* d_state, sdb_stream_t stream);
+/* dfeat = dhead . [w_prob | w_dist]^T, times the features ReLU mask when relu = 1 */
+int sdb_heads_backward(const float* d_feat, const float* d_dhead, long long npix, int cfeat, const float* d_wp,
+                       const float* d_wd, int n_rays, int relu, float* d_dfeat, sdb_stream_t stream);
+/* TF2 Keras Adam over n parameters; alpha = lr * coef[t - 1] with t = d_state[0]; nothing when d_state[2] (skipped step) */
+int sdb_adam_step(float* d_w, const float* d_g, float* d_m, float* d_v, long long n, float lr, float one_minus_b1,
+                  float one_minus_b2, float eps, const float* d_coef, const int* d_state, sdb_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -59,6 +59,26 @@ def _declare(lib):
     lib.sdb_class_head.restype = c_int
     lib.sdb_merge_split.argtypes = [P, P, c_longlong, P, P]
     lib.sdb_merge_split.restype = c_int
+    lib.sdb_conv_wgrad_workspace.argtypes = [c_longlong, c_int, c_int, c_int]
+    lib.sdb_conv_wgrad_workspace.restype = c_longlong
+    lib.sdb_conv_wgrad_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, P, c_longlong, P, P, P]
+    lib.sdb_conv_wgrad_nd.restype = c_int
+    lib.sdb_conv_flip_weights.argtypes = [P, c_int, c_int, c_int, P, P]
+    lib.sdb_conv_flip_weights.restype = c_int
+    lib.sdb_decoder_split.argtypes = [P] + [c_int] * 9 + [P, P, P]
+    lib.sdb_decoder_split.restype = c_int
+    lib.sdb_relu_backward.argtypes = [P, P, c_longlong, P]
+    lib.sdb_relu_backward.restype = c_int
+    lib.sdb_maxpool_backward_nd.argtypes = [P, P] + [c_int] * 9 + [P, P]
+    lib.sdb_maxpool_backward_nd.restype = c_int
+    lib.sdb_stardist_loss_workspace.argtypes = [c_longlong]
+    lib.sdb_stardist_loss_workspace.restype = c_longlong
+    lib.sdb_stardist_loss.argtypes = [P, P, P, P, c_longlong, c_int, c_int, c_float, c_float, c_float, P, P, P, P, P, P]
+    lib.sdb_stardist_loss.restype = c_int
+    lib.sdb_heads_backward.argtypes = [P, P, c_longlong, c_int, P, P, c_int, c_int, P, P]
+    lib.sdb_heads_backward.restype = c_int
+    lib.sdb_adam_step.argtypes = [P, P, P, P, c_longlong, c_float, c_float, c_float, c_float, P, P, P]
+    lib.sdb_adam_step.restype = c_int
     lib.sdb_heads_2d.argtypes = [P, c_longlong, c_int, P, P, P, P, c_int, P, P, P]
     lib.sdb_conv3x3_tc.argtypes = [P, P, c_int, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, c_int, P, P, P]
     lib.sdb_heads_tc.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, P, P, P]

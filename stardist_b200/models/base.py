@@ -6,7 +6,7 @@ Mirrors the prediction half of stardist/models/base.py:
   predict_instances_big (:838-983), thresholds handling (:230-252), _compute_receptive_field
   (:1068-1098), _axes_tile_overlap (:1101-1111), StarDistPadAndCropResizer (:1162-1211),
   optimize_thresholds (:986-1043), _guess_n_tiles (:1046-1055).
-Training and export are out of scope (DESIGN.md).
+Training is in models/train.py; export is out of scope (DESIGN.md).
 
 Differences by design: the network, thresholding, sort, NMS and label painting all run as CUDA
 kernels on tensors that stay in HBM; only the final labels / polygons are copied to the host.
@@ -196,6 +196,11 @@ class StarDistBase:
         if self._net is None:
             self._net = self._build()
         return self._net
+
+    def prepare_for_training(self, optimizer=None):
+        """checks that train() covers this model; only the default optimizer (Adam with train_learning_rate) is supported"""
+        from .train import check_trainable
+        check_trainable(self.config, optimizer)
 
     def save_weights(self, path):
         np.savez(path, **{('%s/kernel' % k): v[0] for k, v in self.weights.items()},

@@ -17,7 +17,7 @@ from .unet_device import UNetDevice2D, UNetDevice2DTC
 
 
 class StarDist2D(StarDistBase):
-    """StarDist2D model (prediction only).
+    """StarDist2D model (prediction and training).
 
     Parameters
     ----------
@@ -143,6 +143,14 @@ class StarDist2D(StarDistBase):
             tuple(p ** self.config.unet_n_depth * g for p, g in zip(self.config.unet_pool, self.config.grid))
         ))
         return tuple(div_by.get(a, 1) for a in query_axes)
+
+    def train(self, X, Y, validation_data, classes='auto', augmenter=None, seed=None, epochs=None, steps_per_epoch=None, workers=1):
+        """Train the network on the device (reference signature; see models/train.py and DESIGN.md 4.2).  Returns a
+        History whose .history holds loss, prob_loss, dist_loss, val_loss, val_prob_loss, val_dist_loss and lr per epoch.
+        `workers` is accepted for compatibility (batches are made on the device); `train_tensorboard` is ignored."""
+        from .train import train
+        return train(self, X, Y, validation_data, classes=classes, augmenter=augmenter, seed=seed, epochs=epochs,
+                     steps_per_epoch=steps_per_epoch, workers=workers)
 
     @property
     def _config_class(self):

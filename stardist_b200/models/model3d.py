@@ -19,7 +19,7 @@ from .unet_device import UNetDeviceND, ResNetDeviceND, UNetDevice3DTC
 
 
 class StarDist3D(StarDistBase):
-    """StarDist3D model (prediction only)."""
+    """StarDist3D model (prediction and training)."""
 
     def __init__(self, config=Config3D(), name=None, basedir='.', **kwargs):
         super().__init__(config, name=name, basedir=basedir, **kwargs)
@@ -180,6 +180,14 @@ class StarDist3D(StarDistBase):
             tuple(p ** self.config.unet_n_depth * g for p, g in zip(self.config.unet_pool, self.config.grid))
         ))
         return tuple(div_by.get(a, 1) for a in query_axes)
+
+    def train(self, X, Y, validation_data, classes='auto', augmenter=None, seed=None, epochs=None, steps_per_epoch=None, workers=1):
+        """Train the network on the device (reference signature; see models/train.py and DESIGN.md 4.2).  Returns a
+        History whose .history holds loss, prob_loss, dist_loss, val_loss, val_prob_loss, val_dist_loss and lr per epoch.
+        `workers` is accepted for compatibility (batches are made on the device); `train_tensorboard` is ignored."""
+        from .train import train
+        return train(self, X, Y, validation_data, classes=classes, augmenter=augmenter, seed=seed, epochs=epochs,
+                     steps_per_epoch=steps_per_epoch, workers=workers)
 
     @property
     def _config_class(self):

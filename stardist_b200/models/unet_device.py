@@ -73,25 +73,33 @@ class UNetDeviceND:
         L.check(lib.sdb_maxpool_nd(L.ptr(x), n, d, h, w, c, int(pz), int(py), int(px), L.ptr(out), L.stream_ptr()))
         return out
 
-    def forward(self, x):
-        """x: float32 [N,(D,)H,W,Cin] on the device -> (prob [N,...], dist [N,...,R])"""
+    def forward(self, x, keep=False):
+        """x: float32 [N,(D,)H,W,Cin] on the device -> (prob [N,...], dist [N,...,R]).
+        keep=True stores in self.saved, per entry of self.layers, what the backward pass reads: for a convolution its
+        inputs (x, x_lo, up) and its output y, for a pooling its input x; self.saved_feat is the heads' input."""
         lib = L.load()
         assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
         skips = {}
         lo, up = None, (1,) * self.nd
         base = None
-        for l in self.layers:
+        saved = [None] * len(self.layers) if keep else None
+        for i, l in enumerate(self.layers):
             kind = l['kind']
             if kind == 'conv':
                 act = l['act']
                 if act not in ('relu', 'linear'):
                     raise NotImplementedError("activation %s" % act)
                 if l['name'] == 'features': base = x
-                x = self._conv(x, lo, l['name'], act == 'relu', up)
+                y = self._conv(x, lo, l['name'], act == 'relu', up)
+                if keep:
+                    saved[i] = dict(x=x, lo=lo, up=up, y=y)
+                x = y
                 lo, up = None, (1,) * self.nd
             elif kind == 'pool':
                 if 'save_skip' in l:
                     skips[l['save_skip']] = x
+                if keep:
+                    saved[i] = dict(x=x)
                 x = self._pool(x, l['pool'])
             elif kind == 'up':
                 lo, up = x, tuple(l['pool'])           # consumed by the next conv together with the skip
@@ -99,6 +107,8 @@ class UNetDeviceND:
             elif kind == 'head':
                 break
         feat = x
+        if keep:
+            self.saved, self.saved_feat = saved, feat
         cf = feat.shape[-1]
         npix = int(np.prod(feat.shape[:-1]))
         R = self.config.n_rays
