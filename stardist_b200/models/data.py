@@ -1,8 +1,19 @@
 """Training batches on the device: StarDistData2D / StarDistData3D (stardist/models/base.py:129-225, model2d.py:29-120,
 model3d.py:30-127), the data generators a StarDist training loop consumes.
 
-The images and masks are uploaded once at construction and stay resident.  A batch is drawn on the host (the random
-stream: which images, foreground or not, which rank among the valid positions) and built on the device:
+X / Y given as lists, tuples or arrays are uploaded once at construction and stay resident.  Any other X / Y with len()
+and integer __getitem__ returning arrays (a keras.utils.Sequence-like loader, a list-like wrapper over files, zarr-backed
+arrays) is lazy: construction reads X[0] (twice when it has a channel axis) and uploads nothing, and every batch reads
+exactly what the reference's __getitem__ reads, in its order (LazyReads), so a loader that draws from np.random itself
+leaves the global stream, and therefore the batches, as the reference does.  Each item read goes up through a pinned
+staging buffer and is relabelled on the device; the foreground mask and prefix of an image come from the read the
+reference takes its valid positions from, and are kept on the device (1 byte per pixel plus the prefix) only with
+sample_ind_cache=True.  Nothing else of a lazy image outlives its batch.  The resident path's construction checks (shapes,
+image size, channel count, integer masks and their label range) are made on every read, before the read is uploaded;
+class tables are built per item.  A lazy X item becomes float32 like a resident one (the reference keeps its dtype).
+
+A batch is drawn on the host (the random stream: which images, foreground or not, which rank among the valid positions)
+and built on the device:
 - the rank of every item becomes a patch position (csrc/traindata.cu: sdb_sample_select, over the foreground mask and
   prefix counts of sdb_fg_valid_index for the foreground-restricted draws);
 - one gather copies the X channels and label crops of the whole batch, clamps negative labels and marks them at the grid
@@ -12,15 +23,16 @@ stream: which images, foreground or not, which rank among the valid positions) a
 The reference's values are those of its `cpp` / scipy path (gputools and the `edt` package give different numbers).
 
 Labels are handled through a per-image sequential relabelling (ascending order, negative labels -> 0) made at
-construction: each item's labels are offset so that no two items share one, which sizes edt_prob's per-label maxima and
-the class tables without reading anything back.  Star distances see the clamped original labels (compared by their low
-16 bits, as the reference's uint16 cast does).
+construction (for a lazy dataset: per item read): each item's labels are offset so that no two items share one, which
+sizes edt_prob's per-label maxima and the class tables without reading anything back.  Star distances see the clamped
+original labels (compared by their low 16 bits, as the reference's uint16 cast does).
 
-Differences from the reference, all raised before anything is launched: `shape_completion=True` and lazy (non-list) X / Y
-raise NotImplementedError / ValueError; class ids are checked when the generator is made (the reference checks them per
-batch), and a dict key 0 (which would class the background) is NotImplementedError.  A label of a patch that has no class
-in the dict raises the reference's ValueError when that batch is made.  X is returned as float32 even when an augmenter
-returns another float type.
+Differences from the reference, all raised before anything is launched: `shape_completion=True` raises
+NotImplementedError, and an X / Y without len() / __getitem__ ValueError; class ids are checked when the generator is made
+(the reference checks them per batch), and a dict key 0 (which would class the background) is NotImplementedError.  Two
+reads of one lazy image with different shapes (the reference would crop one at positions valid for the other) raise
+ValueError.  A label of a patch that has no class in the dict raises the reference's ValueError when that batch is made.
+X is returned as float32 even when an augmenter returns another float type.
 """
 import random, threading, warnings
 import numpy as np
@@ -89,18 +101,23 @@ class RollingSequence:
         return index[sl]
 
 
-def plan_batch(seq, i, foreground_prob, n_valid):
+def plan_batch(seq, i, foreground_prob, n_valid, read=None):
     """the host side of batch i: (image indices, [(image, foreground_only, rank)]), drawing from np.random with exactly the
     calls of the reference's __getitem__ (StarDistDataBase.get_valid_inds, sample_patches).  n_valid(k, foreground_only)
-    is the number of valid positions of image k."""
+    is the number of valid positions of image k; it is called once per index lookup of the reference's get_valid_inds
+    (twice when an image without foreground falls back to foreground_prob=0).  read(k), when given, is called at the start
+    of every item, where the reference reads Y[k] and X[k] for sample_patches."""
     idx = seq.batch(i)
     plan = []
     for k in idx:
         k = int(k)
+        if read is not None:
+            read(k)
         fg = bool(np.random.uniform() < foreground_prob)
-        if fg and n_valid(k, True) == 0:
-            fg = bool(np.random.uniform() < 0)             # no foreground: get_valid_inds(k, foreground_prob=0)
         n = n_valid(k, fg)
+        if fg and n == 0:
+            fg = bool(np.random.uniform() < 0)             # no foreground: get_valid_inds(k, foreground_prob=0)
+            n = n_valid(k, fg)
         if n == 0:
             raise ValueError("no regions to sample from!")
         rank = choice(range(n), 1, replace=(n < 1))[0]
@@ -127,6 +144,68 @@ def _class_code(cls, n_classes):
     raise ValueError(f"Wrong class id '{cls}' (for n_classes={n_classes})")
 
 
+def _is_resident(X):
+    return isinstance(X, (np.ndarray, tuple, list))
+
+
+def _check_mask(y):
+    if not np.issubdtype(y.dtype, np.integer):
+        raise ValueError("masks must be integer label images, got %s" % y.dtype)
+    if y.size and (int(y.min()) < np.iinfo(np.int32).min or int(y.max()) > _MAX_LABEL):
+        raise ValueError("labels must fit int32 and lie below 2^30 (labels above 2^30 - 1 are not supported)")
+
+
+class LazyReads:
+    """The reads of a lazy X / Y (any object with len() and integer __getitem__ returning arrays), in the reference's order
+    and number, so that a sequence drawing from np.random itself leaves the global stream as the reference does.  Per item
+    of a batch: Y[k], then X[k] (the arguments of sample_patches); then one more Y[k] whenever the reference's
+    _ind_cache_fg / _ind_cache_all has no entry for k (StarDistDataBase.get_valid_inds), including the fallback to
+    foreground_prob=0 of an image without foreground.  The key sets of those two caches are kept here, with what the
+    reference would keep for them: the shape and valid-position count, and fg_index's payload for the foreground ones.
+
+    check_item(x, y) -> (x, y) and check_mask(y) -> y make the resident path's construction checks on every read;
+    fg_index(y) -> (count, payload) computes the foreground-restricted valid positions of a mask read."""
+
+    def __init__(self, X, Y, patch_size, sample_ind_cache, check_item, check_mask, fg_index):
+        self.X, self.Y = X, Y
+        self.patch_size, self.sample_ind_cache = tuple(patch_size), bool(sample_ind_cache)
+        self.check_item, self.check_mask, self.fg_index = check_item, check_mask, fg_index
+        self.cache = {True: {}, False: {}}
+
+    def plan(self, seq, i, foreground_prob):
+        """-> (image indices, [(image, foreground_only, rank)], [[x, y, fg payload] per item]) for batch i"""
+        items = []
+
+        def read(k):
+            y = self.Y[k]
+            x = self.X[k]
+            items.append(list(self.check_item(x, y)) + [None])
+
+        def n_valid(k, fg):
+            item = items[-1]
+            cache = self.cache[fg]
+            if k in cache:
+                shape, n, payload = cache[k]
+            else:
+                y = self.check_mask(self.Y[k])
+                shape = y.shape
+            if shape != item[1].shape:
+                raise ValueError("images and masks should have corresponding shapes/dimensions")
+            if k not in cache:
+                if fg:
+                    n, payload = self.fg_index(y)
+                else:
+                    n, payload = int(np.prod([s - p + 1 for s, p in zip(shape, self.patch_size)])), None
+                if self.sample_ind_cache:
+                    cache[k] = (shape, n, payload)
+            if fg:
+                item[2] = payload
+            return n
+
+        idx, plan = plan_batch(seq, i, foreground_prob, n_valid, read)
+        return idx, plan, items
+
+
 # ---------------------------------------------------------------------------------------------------- the generators
 
 class _StarDistDataDevice(RollingSequence):
@@ -138,11 +217,13 @@ class _StarDistDataDevice(RollingSequence):
                  maxfilter_patch_size=None, keras_kwargs=None):
         from ..geometry.distances import _check_grid, walk_bound
         from ..labelprep import _sampling
-        if not (isinstance(X, (np.ndarray, tuple, list)) and isinstance(Y, (np.ndarray, tuple, list))):
-            raise ValueError("X and Y must be lists, tuples or arrays of images (lazy sequences are not supported)")
+        resident = _is_resident(X) and _is_resident(Y)
+        if not resident and not all(hasattr(v, "__len__") and hasattr(v, "__getitem__") for v in (X, Y)):
+            raise ValueError("X and Y must be lists, tuples or arrays of images, or sequences with len() and __getitem__")
         super().__init__(data_size=len(X), batch_size=batch_size, length=length, shuffle=True, keras_kwargs=keras_kwargs)
-        X = [np.asarray(x).astype(np.float32, copy=False) for x in X]
-        Y = [np.asarray(y) for y in Y]
+        if resident:
+            X = [np.asarray(x).astype(np.float32, copy=False) for x in X]
+            Y = [np.asarray(y) for y in Y]
         len(X) == len(Y) and len(X) > 0 or _raise(ValueError("X and Y can't be empty and must have same length"))
         if classes is None:
             classes = (None,) * len(X)
@@ -154,16 +235,18 @@ class _StarDistDataDevice(RollingSequence):
         nD = len(patch_size)
         if nD != ndim:
             raise AssertionError("patch_size must have %d values" % ndim)
-        x_ndim = X[0].ndim
+        x_ndim = np.ndim(X[0])                              # a lazy X is read here, and once more for its channel count
         if x_ndim not in (nD, nD + 1):
             raise AssertionError("images must have %d or %d dimensions" % (nD, nD + 1))
-        all(y.ndim == nD and x.ndim == x_ndim and x.shape[:nD] == y.shape for x, y in zip(X, Y)) or _raise(
-            ValueError("images and masks should have corresponding shapes/dimensions"))
-        all(all(s >= p for s, p in zip(x.shape[:nD], patch_size)) for x in X) or _raise(
-            ValueError("Some images are too small for given patch_size {patch_size}".format(patch_size=patch_size)))
-        self.n_channel = None if x_ndim == nD else X[0].shape[-1]
-        if self.n_channel is not None and not all(x.shape[-1] == self.n_channel for x in X):
-            raise AssertionError("all images must have the same number of channels")
+        self.n_channel = None if x_ndim == nD else int(np.shape(X[0])[-1])
+        self._x_ndim = x_ndim
+        if resident:
+            all(y.ndim == nD and x.ndim == x_ndim and x.shape[:nD] == y.shape for x, y in zip(X, Y)) or _raise(
+                ValueError("images and masks should have corresponding shapes/dimensions"))
+            all(all(s >= p for s, p in zip(x.shape[:nD], patch_size)) for x in X) or _raise(
+                ValueError("Some images are too small for given patch_size {patch_size}".format(patch_size=patch_size)))
+            if self.n_channel is not None and not all(x.shape[-1] == self.n_channel for x in X):
+                raise AssertionError("all images must have the same number of channels")
         if not (0 <= foreground_prob <= 1):
             raise AssertionError("foreground_prob must lie in [0, 1]")
         if augmenter is None:
@@ -172,11 +255,9 @@ class _StarDistDataDevice(RollingSequence):
         else:
             callable(augmenter) or _raise(ValueError("augmenter must be None or callable"))
             self._augment = True
-        for y in Y:
-            if not np.issubdtype(y.dtype, np.integer):
-                raise ValueError("masks must be integer label images, got %s" % y.dtype)
-            if y.size and (int(y.min()) < np.iinfo(np.int32).min or int(y.max()) > _MAX_LABEL):
-                raise ValueError("labels must fit int32 and lie below 2^30 (labels above 2^30 - 1 are not supported)")
+        if resident:
+            for y in Y:
+                _check_mask(y)
         self._n_classes_checked(n_classes, classes)
         maxf = patch_size if maxfilter_patch_size is None else maxfilter_patch_size
         maxf = tuple(int(v) for v in np.broadcast_to(np.asarray(maxf), (ndim,)))
@@ -186,7 +267,7 @@ class _StarDistDataDevice(RollingSequence):
         walk_bound(self._table, patch_size)
         self._sampling = _sampling(anisotropy, ndim)
 
-        self.ndim, self.X_shapes = ndim, [y.shape for y in Y]
+        self.ndim, self.X_shapes = ndim, ([y.shape for y in Y] if resident else None)
         self.n_rays, self.patch_size, self.grid = int(n_rays), tuple(patch_size), tuple(grid)
         self.ss_grid = (slice(None),) + tuple(slice(0, None, g) for g in grid)
         self.n_classes, self.classes = n_classes, classes
@@ -203,11 +284,17 @@ class _StarDistDataDevice(RollingSequence):
             self._zoom_shape = tuple(n for n, _ in zs)
             self._zoom_index = np.concatenate([ix for _, ix in zs]).astype(np.int32)
 
-        # resident dataset: X float32 [..., C], Y int32, the sequential relabelling of Y and its label count
         import torch
         from ..labelprep import _relabel
         L.require_cuda()
         self._X, self._Y, self._seq, self._n, self._cls = [], [], [], [], []
+        self._fg = {}
+        self._lazy, self._stage, self._stage_done = None, None, None
+        if not resident:
+            # lazy dataset: nothing is read or uploaded until a batch needs it
+            self._lazy = LazyReads(X, Y, self.patch_size, sample_ind_cache, self._check_item, self._check_valid_mask, self._fg_index)
+            return
+        # resident dataset: X float32 [..., C], Y int32, the sequential relabelling of Y and its label count
         for k, (x, y) in enumerate(zip(X, Y)):
             xs = x if self.n_channel is not None else x[..., None]
             self._X.append(torch.from_numpy(np.ascontiguousarray(xs)).to("cuda"))
@@ -216,7 +303,6 @@ class _StarDistDataDevice(RollingSequence):
             self._Y.append(yt); self._seq.append(seq); self._n.append(n)
             if n_classes is not None:
                 self._cls.append(self._class_table(classes[k], labels.cpu().numpy()))
-        self._fg = {}
 
     # -------------------------------------------------------------------------------------------- classes
     @staticmethod
@@ -252,17 +338,79 @@ class _StarDistDataDevice(RollingSequence):
             return int(np.prod([s - p + 1 for s, p in zip(shape, self.patch_size)]))
         if self.sample_ind_cache and k in self._fg:
             return self._fg[k][2]
+        m = self._fg_valid_index(self._Y[k])
+        with self.lock:
+            self._fg[k] = m
+        return m[2]
+
+    def _fg_valid_index(self, y):
+        """sdb_fg_valid_index of a CUDA int32 mask: (foreground mask uint8, int64 prefix counts per valid row, count)"""
         import ctypes, torch
         lib = L.require_cuda()
+        shape = tuple(y.shape)
         rows = int(np.prod([s - p + 1 for s, p in zip(shape[:-1], self.patch_size[:-1])]))
         mask = torch.empty(shape, dtype=torch.uint8, device="cuda")
         prefix = torch.empty(rows + 1, dtype=torch.int64, device="cuda")
         n = ctypes.c_longlong(0)
-        L.check(lib.sdb_fg_valid_index(L.ptr(self._Y[k]), self.ndim, L.iarr(shape), L.iarr(self._maxf), L.iarr(self.patch_size),
+        L.check(lib.sdb_fg_valid_index(L.ptr(y), self.ndim, L.iarr(shape), L.iarr(self._maxf), L.iarr(self.patch_size),
                                        L.ptr(mask), L.ptr(prefix), ctypes.byref(n), L.stream_ptr()))
-        with self.lock:
-            self._fg[k] = (mask, prefix, int(n.value))
-        return int(n.value)
+        return mask, prefix, int(n.value)
+
+    # -------------------------------------------------------------------------------------------- lazy X / Y
+    def _check_item(self, x, y):
+        """an item read from a lazy X / Y, with the checks the resident path makes at construction"""
+        x, y = np.asarray(x), np.asarray(y)
+        nD, p = self.ndim, self.patch_size
+        y.ndim == nD and x.ndim == self._x_ndim and x.shape[:nD] == y.shape or _raise(
+            ValueError("images and masks should have corresponding shapes/dimensions"))
+        all(s >= q for s, q in zip(y.shape, p)) or _raise(
+            ValueError("Some images are too small for given patch_size {patch_size}".format(patch_size=p)))
+        if self.n_channel is not None and x.shape[-1] != self.n_channel:
+            raise AssertionError("all images must have the same number of channels")
+        _check_mask(y)
+        return x, y
+
+    def _check_valid_mask(self, y):
+        """a mask read for the valid positions only (StarDistDataBase.get_valid_inds)"""
+        y = np.asarray(y)
+        y.ndim == self.ndim or _raise(ValueError("images and masks should have corresponding shapes/dimensions"))
+        _check_mask(y)
+        return y
+
+    def _fg_index(self, y):
+        mask, prefix, n = self._fg_valid_index(self._upload(y, np.int32))
+        return n, (mask, prefix)
+
+    def _upload(self, a, dtype):
+        """numpy array -> new CUDA tensor of dtype (the value conversion of astype), through the pinned staging buffer"""
+        import torch
+        dtype = np.dtype(dtype)
+        nbytes = a.size * dtype.itemsize
+        if self._stage_done is not None:
+            self._stage_done.synchronize()                 # the previous upload has left the buffer
+        if self._stage is None or self._stage.numel() < nbytes:
+            self._stage = None
+            self._stage = torch.empty(max(nbytes, 1), dtype=torch.uint8, pin_memory=True)
+            self._stage_done = torch.cuda.Event()
+        h = self._stage[:nbytes].view(getattr(torch, dtype.name)).view(a.shape)
+        np.copyto(h.numpy(), a, casting='unsafe')
+        d = torch.empty(a.shape, dtype=h.dtype, device="cuda")
+        d.copy_(h, non_blocking=True)
+        self._stage_done.record()
+        return d
+
+    def _lazy_items(self, plan, items):
+        """the uploaded items of a lazy batch, as _batch reads the resident ones: (X, Y, sequential Y, label count, class
+        table, foreground mask and prefix or None) per item"""
+        from ..labelprep import _relabel
+        out = []
+        for (k, fg, _), (x, y, fgm) in zip(plan, items):
+            xt = self._upload(x if self.n_channel is not None else x[..., None], np.float32)
+            yt = self._upload(y, np.int32)
+            seq, n, labels, _, _ = _relabel(yt)
+            cls = self._class_table(self.classes[k], labels.cpu().numpy()) if self.n_classes is not None else None
+            out.append((xt, yt, seq, n, cls, fgm if fg else None))
+        return out
 
     def _items(self, rows):
         """int64 [B][10] item table (csrc/traindata.cu) on the device"""
@@ -275,19 +423,25 @@ class _StarDistDataDevice(RollingSequence):
         per-item label min / max) for _finish"""
         import torch
         lib = L.require_cuda()
-        idx, plan = plan_batch(self, i, self.foreground_prob, self._n_valid)
+        if self._lazy is None:
+            idx, plan = plan_batch(self, i, self.foreground_prob, self._n_valid)
+            res = [(self._X[k], self._Y[k], self._seq[k], self._n[k], self._cls[k] if self._cls else None, self._fg[k] if fg else None)
+                   for k, fg, _ in plan]
+        else:
+            idx, plan, read = self._lazy.plan(self, i, self.foreground_prob)
+            res = self._lazy_items(plan, read)
+            del read
         B, nd, p, g = len(plan), self.ndim, self.patch_size, self.grid
         C = 1 if self.n_channel is None else self.n_channel
         pg = tuple((a - 1) // b + 1 for a, b in zip(p, g))
         P = int(np.prod(p))
         dev = "cuda"
         rows, off = [], 0
-        for k, fg, rank in plan:
-            m = self._fg[k] if fg else None
-            shape3 = (1,) * (3 - nd) + tuple(self.X_shapes[k])
-            rows.append([self._X[k].data_ptr(), self._Y[k].data_ptr(), self._seq[k].data_ptr(), m[0].data_ptr() if m else 0,
+        for (k, fg, rank), (xk, yk, seqk, nk, _, m) in zip(plan, res):
+            shape3 = (1,) * (3 - nd) + tuple(yk.shape)
+            rows.append([xk.data_ptr(), yk.data_ptr(), seqk.data_ptr(), m[0].data_ptr() if m else 0,
                          m[1].data_ptr() if m else 0, rank, off, *shape3])
-            off += self._n[k]
+            off += nk
         items = self._items(rows)
         pos = torch.empty((B, 3), dtype=torch.int32, device=dev)
         L.check(lib.sdb_sample_select(L.ptr(items), nd, B, L.iarr(p), L.ptr(pos), L.stream_ptr()))
@@ -296,7 +450,7 @@ class _StarDistDataDevice(RollingSequence):
         classes_on = self.n_classes is not None
         cls_table = None
         if classes_on:
-            cls_table = np.concatenate([np.zeros(1, np.int32)] + [self._cls[k][1:] for k, _, _ in plan])
+            cls_table = np.concatenate([np.zeros(1, np.int32)] + [r[4][1:] for r in res])
 
         status = torch.zeros(1 + 2 * B, dtype=torch.int32, device=dev)
         x = torch.empty((B,) + p + (C,), dtype=torch.float32, device=dev)
@@ -335,6 +489,7 @@ class _StarDistDataDevice(RollingSequence):
         d_cls = torch.from_numpy(cls_table).to(dev) if classes_on else None
         L.check(lib.sdb_train_gather(L.ptr(items), L.ptr(pos), nd, B, L.iarr(p), C, L.iarr(g), L.ptr(d_cls), L.ptr(x), L.ptr(yc), L.ptr(ys),
                                      L.ptr(ye), L.ptr(neg), L.ptr(status), 1, L.stream_ptr()))
+        del res                # a lazy batch's images are not read past the gather (their memory is reused in stream order)
         R = self.n_rays
         dam = torch.empty((B,) + pg + (R + 1,), dtype=torch.float32, device=dev)
         prob = torch.empty((B,) + pg + (1,), dtype=torch.float32, device=dev)

@@ -184,6 +184,8 @@ class StarDist3D(StarDistBase):
     def train(self, X, Y, validation_data, classes='auto', augmenter=None, seed=None, epochs=None, steps_per_epoch=None, workers=1):
         """Train the network on the device (reference signature; see models/train.py and DESIGN.md 4.2).  Returns a
         History whose .history holds loss, prob_loss, dist_loss, val_loss, val_prob_loss, val_dist_loss and lr per epoch.
+        X, Y and the two of validation_data are lists, tuples or arrays of images, or lazy sequences (len() and
+        __getitem__ returning arrays) read batch by batch (models/data.py).
         `workers` is accepted for compatibility (batches are made on the device); `train_tensorboard` is ignored."""
         from .train import train
         return train(self, X, Y, validation_data, classes=classes, augmenter=augmenter, seed=seed, epochs=epochs,

@@ -296,7 +296,8 @@ class History:
 # ------------------------------------------------------------------------------------------------------ train()
 def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=None, epochs=None, steps_per_epoch=None, workers=1,
           optimizer=None):
-    """StarDist2D.train / StarDist3D.train (stardist/models/model2d.py:352-481, model3d.py): returns a History"""
+    """StarDist2D.train / StarDist3D.train (stardist/models/model2d.py:352-481, model3d.py): returns a History.  X, Y and
+    validation_data's X, Y may be lazy sequences; they go to the generators as given, and the validation patches are made once."""
     config = model.config
     check_trainable(config, optimizer)
     if classes != 'auto' and classes is not None:
