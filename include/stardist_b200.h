@@ -420,6 +420,17 @@ int sdb_stardist_loss(const float* d_prob, const float* d_dist, const float* d_p
 /* dfeat = dhead . [w_prob | w_dist]^T, times the features ReLU mask when relu = 1 */
 int sdb_heads_backward(const float* d_feat, const float* d_dhead, long long npix, int cfeat, const float* d_wp,
                        const float* d_wd, int n_rays, int relu, float* d_dfeat, sdb_stream_t stream);
+/* Weighted categorical cross-entropy of multi-class models (DESIGN.md 4.2): s = softmax output [npix][n_out], targets
+ * prob_class t [npix][n_out] (all channels < 0 on ignored pixels), class weights d_class_w [n_out] on the device, n_out =
+ * n_classes + 1 <= 32.  Writes *d_out_class = L_class, adds w2 * L_class to *d_total (the loss sdb_stardist_loss wrote) and, if
+ * d_dz is not NULL, dz [npix][n_out] = dL/d(softmax logits).  d_work holds sdb_stardist_class_loss_workspace(npix) bytes. */
+long long sdb_stardist_class_loss_workspace(long long npix);
+int sdb_stardist_class_loss(const float* d_s, const float* d_t, long long npix, int n_out, const float* d_class_w, float w2,
+                            void* d_work, float* d_dz, float* d_total, float* d_out_class, sdb_stream_t stream);
+/* dfeat (+)= dz . W^T with W [cfeat][n_out] the prob_class kernel, times the ReLU mask of feat when relu = 1; accumulate = 1 adds
+ * to d_dfeat instead of overwriting it */
+int sdb_class_head_backward(const float* d_feat, const float* d_dz, long long npix, int cfeat, const float* d_w, int n_out,
+                            int relu, int accumulate, float* d_dfeat, sdb_stream_t stream);
 /* TF2 Keras Adam over n parameters; alpha = lr * coef[t - 1] with t = d_state[0]; nothing when d_state[2] (skipped step) */
 int sdb_adam_step(float* d_w, const float* d_g, float* d_m, float* d_v, long long n, float lr, float one_minus_b1,
                   float one_minus_b2, float eps, const float* d_coef, const int* d_state, sdb_stream_t stream);

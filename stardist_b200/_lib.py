@@ -77,6 +77,12 @@ def _declare(lib):
     lib.sdb_stardist_loss.restype = c_int
     lib.sdb_heads_backward.argtypes = [P, P, c_longlong, c_int, P, P, c_int, c_int, P, P]
     lib.sdb_heads_backward.restype = c_int
+    lib.sdb_stardist_class_loss_workspace.argtypes = [c_longlong]
+    lib.sdb_stardist_class_loss_workspace.restype = c_longlong
+    lib.sdb_stardist_class_loss.argtypes = [P, P, c_longlong, c_int, P, c_float, P, P, P, P, P]
+    lib.sdb_stardist_class_loss.restype = c_int
+    lib.sdb_class_head_backward.argtypes = [P, P, c_longlong, c_int, P, c_int, c_int, c_int, P, P]
+    lib.sdb_class_head_backward.restype = c_int
     lib.sdb_adam_step.argtypes = [P, P, P, P, c_longlong, c_float, c_float, c_float, c_float, P, P, P]
     lib.sdb_adam_step.restype = c_int
     lib.sdb_heads_2d.argtypes = [P, c_longlong, c_int, P, P, P, P, c_int, P, P, P]

@@ -1,6 +1,6 @@
 // unet_train.cu -- fp32 CUDA-core kernels of the U-Net training step (NHWC / NDHWC): weight gradients of the
 // 3^d / 1^d convolutions, the decoder split, ReLU and max-pool backward, the StarDist loss with its head gradient,
-// the 1x1 head input gradient and Adam.  The input gradient of the 3^d convolutions is not here: it is the forward
+// the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients and Adam.  The input gradient of the 3^d convolutions is not here: it is the forward
 // kernel of unet_simt.cu (sdb_conv3_nd) run on dY with the spatially flipped, Cin/Cout-transposed kernel written by
 // sdb_conv_flip_weights.
 //
@@ -318,6 +318,58 @@ __global__ void k_loss_final(const double* __restrict__ partial, int nb, long lo
   }
 }
 
+// ------------------------------------------------------------------------------------------ class loss
+// Weighted categorical cross-entropy of the softmax output s [npix][C] against prob_class t [npix][C] (base.py:108-126):
+// S = sum_k (s_k + eps), q_k = s_k / S, c_k = clip(q_k, eps, 1 - eps), l = -sum_k w_k [t_k >= 0] t_k log c_k.  When dz !=
+// nullptr it receives dL/dz_j = (w2 / npix) s_j (b_j - sum_i s_i b_i), the softmax backward of b_j = a_j / S - (sum_k a_k s_k) / S^2,
+// a_k = -w_k [t_k >= 0] t_k / q_k where eps <= q_k <= 1 - eps (the clip passes no gradient outside).  One thread per pixel.
+constexpr int CLS_MAX = 32;              // n_classes + 1, as in sdb_class_head
+
+__global__ void __launch_bounds__(256) k_class_loss(const float* __restrict__ s, const float* __restrict__ t, long long npix, int C,
+                                                    const float* __restrict__ cw, float w2, long long per_block, float* __restrict__ dz,
+                                                    double* __restrict__ partial) {
+  __shared__ float sw[CLS_MAX];
+  if (threadIdx.x < C) sw[threadIdx.x] = cw[threadIdx.x];
+  __syncthreads();
+  const float gs = w2 / (float)npix;
+  double v[1] = {0.0};
+  const long long b0 = (long long)blockIdx.x * per_block, b1 = llmin(npix, b0 + per_block);
+  for (long long p = b0 + threadIdx.x; p < b1; p += 256) {
+    const float* sp = s + p * C;
+    const float* tp = t + p * C;
+    float S = 0.f;
+    for (int k = 0; k < C; ++k) S += sp[k] + KEPS;
+    float l = 0.f, A = 0.f, a[CLS_MAX];
+    for (int k = 0; k < C; ++k) {
+      const float q = sp[k] / S, tk = tp[k];
+      const float c = fminf(fmaxf(q, KEPS), 1.f - KEPS);
+      const float wt = tk >= 0.f ? sw[k] * tk : 0.f;
+      l += wt * logf(c);
+      a[k] = (q >= KEPS && q <= 1.f - KEPS) ? -wt / q : 0.f;
+      A += a[k] * sp[k];
+    }
+    v[0] -= (double)l;
+    if (dz) {
+      const float AS2 = A / (S * S);
+      float sb = 0.f;
+      for (int k = 0; k < C; ++k) { a[k] = a[k] / S - AS2; sb += sp[k] * a[k]; }
+      for (int k = 0; k < C; ++k) dz[p * C + k] = gs * (sp[k] * (a[k] - sb));
+    }
+  }
+  block_reduce_store<1>(v, partial);
+}
+
+// out_class = L_class = sum / npix; total += w2 * L_class (total: the loss sdb_stardist_loss wrote)
+__global__ void k_class_loss_final(const double* __restrict__ partial, int nb, long long npix, float w2, float* __restrict__ total,
+                                   float* __restrict__ out_class) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  double a = 0.0;
+  for (int i = 0; i < nb; ++i) a += partial[i];
+  const float lc = (float)(a / (double)npix);
+  *out_class = lc;
+  *total = __fadd_rn(*total, __fmul_rn(w2, lc));
+}
+
 // ------------------------------------------------------------------------------------------ heads backward
 // dfeat[p][f] = sum_o dhead[p][o] * W[f][o] (W[f][0] = w_prob[f], W[f][1 + r] = w_dist[f][r]), o in order, then the ReLU
 // mask of the features layer's output.  32 pixels per CTA.
@@ -346,6 +398,37 @@ __global__ void __launch_bounds__(128) k_heads_backward(const float* __restrict_
       for (int o = 0; o < NO; ++o) acc = fmaf(sG[px * NO + o], sW[o * cf + f], acc);
       if (relu && !(feat[p * cf + f] > 0.f)) acc = 0.f;
       dfeat[p * cf + f] = acc;
+    }
+  }
+}
+
+// dfeat[p][f] (+)= sum_o dz[p][o] * W[f][o] (W [cf][C], the prob_class kernel), o in order, times the ReLU mask of feat when
+// relu = 1.  accumulate = 1 adds the class branch's share to a tensor the heads' backward has written (both read one input).
+// 32 pixels per CTA.
+__global__ void __launch_bounds__(128) k_class_head_backward(const float* __restrict__ feat, const float* __restrict__ dz, long long npix,
+                                                             int cf, const float* __restrict__ w, int C, int relu, int accumulate,
+                                                             float* __restrict__ dfeat) {
+  extern __shared__ float sm[];
+  float* sW = sm;                 // [C][cf]
+  float* sG = sW + C * cf;        // [32][C]
+  for (int e = threadIdx.x; e < C * cf; e += blockDim.x) {
+    const int o = e / cf, f = e % cf;
+    sW[e] = w[(size_t)f * C + o];
+  }
+  const long long p0 = (long long)blockIdx.x * 32;
+  for (int e = threadIdx.x; e < 32 * C; e += blockDim.x) {
+    const long long p = p0 + e / C;
+    sG[e] = p < npix ? dz[p0 * C + e] : 0.f;
+  }
+  __syncthreads();
+  for (int px = 0; px < 32; ++px) {
+    const long long p = p0 + px;
+    if (p >= npix) break;
+    for (int f = threadIdx.x; f < cf; f += blockDim.x) {
+      float acc = 0.f;
+      for (int o = 0; o < C; ++o) acc = fmaf(sG[px * C + o], sW[o * cf + f], acc);
+      if (relu && !(feat[p * cf + f] > 0.f)) acc = 0.f;
+      dfeat[p * cf + f] = accumulate ? __fadd_rn(dfeat[p * cf + f], acc) : acc;
     }
   }
 }
@@ -466,6 +549,35 @@ extern "C" int sdb_heads_backward(const float* d_feat, const float* d_dhead, lon
   static bool attr_set = false;
   if (!attr_set) { SDB_CUDA(cudaFuncSetAttribute(k_heads_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr_set = true; }
   SDB_LAUNCH(k_heads_backward, cdiv(npix, 32), 128, smem, st, d_feat, d_dhead, npix, cfeat, d_wp, d_wd, n_rays, relu, d_dfeat);
+  return 0;
+}
+
+extern "C" long long sdb_stardist_class_loss_workspace(long long npix) {
+  return (long long)loss_blocks(npix) * (long long)sizeof(double);
+}
+
+extern "C" int sdb_stardist_class_loss(const float* d_s, const float* d_t, long long npix, int n_out, const float* d_class_w, float w2,
+                                       void* d_work, float* d_dz, float* d_total, float* d_out_class, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (npix < 1 || n_out < 1 || n_out > CLS_MAX) { sdb::set_error("stardist_class_loss: npix >= 1 and n_classes + 1 in [1,32] required"); return 1; }
+  const int nb = loss_blocks(npix);
+  const long long per = (npix + nb - 1) / nb;
+  double* part = (double*)d_work;
+  SDB_LAUNCH(k_class_loss, nb, 256, 0, st, d_s, d_t, npix, n_out, d_class_w, w2, per, d_dz, part);
+  SDB_LAUNCH(k_class_loss_final, 1, 32, 0, st, part, nb, npix, w2, d_total, d_out_class);
+  return 0;
+}
+
+extern "C" int sdb_class_head_backward(const float* d_feat, const float* d_dz, long long npix, int cfeat, const float* d_w, int n_out,
+                                       int relu, int accumulate, float* d_dfeat, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (npix <= 0) return 0;
+  if (n_out < 1 || n_out > CLS_MAX || cfeat < 1) { sdb::set_error("class_head_backward: n_classes + 1 must be in [1,32]"); return 1; }
+  const size_t smem = (size_t)(n_out * cfeat + 32 * n_out) * sizeof(float);
+  if (smem > 200 * 1024) { sdb::set_error("class_head_backward: n_classes * features too large"); return 1; }
+  static bool attr_set = false;
+  if (!attr_set) { SDB_CUDA(cudaFuncSetAttribute(k_class_head_backward, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr_set = true; }
+  SDB_LAUNCH(k_class_head_backward, cdiv(npix, 32), 128, smem, st, d_feat, d_dz, npix, cfeat, d_w, n_out, relu, accumulate, d_dfeat);
   return 0;
 }
 

@@ -107,6 +107,11 @@ class StarDistPadAndCropResizer:
         return np.where(np.all(points < bounds, 1))
 
 
+class AutoClassesNotSupported(ValueError, NotImplementedError):
+    """classes='auto' for n_classes > 1: the reference's ValueError, also a NotImplementedError because this project reported
+    it as such before multi-class training existed"""
+
+
 class StarDistBase:
     """Common prediction logic of StarDist2D / StarDist3D."""
 
@@ -190,6 +195,23 @@ class StarDistBase:
 
     def _is_multiclass(self):
         return self.config.n_classes is not None
+
+    def _parse_classes_arg(self, classes, length):
+        """the classes tuple for train() (base.py:262-284): 'auto' -> None without n_classes, (1,) * length for n_classes == 1;
+        a tuple, list or array must have the given length"""
+        if isinstance(classes, str):
+            classes == "auto" or _raise(ValueError(f"classes = '{classes}': only 'auto' supported as string argument for classes"))
+            if self.config.n_classes is None:
+                classes = None
+            elif self.config.n_classes == 1:
+                classes = (1,) * length
+            else:
+                raise AutoClassesNotSupported("using classes = 'auto' for n_classes > 1 not supported")
+        elif isinstance(classes, (tuple, list, np.ndarray)):
+            len(classes) == length or _raise(ValueError(f"len(classes) should be {length}!"))
+        else:
+            raise ValueError("classes should either be 'auto' or a list of scalars/label dicts")
+        return classes
 
     @property
     def net(self):

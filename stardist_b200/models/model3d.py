@@ -183,9 +183,11 @@ class StarDist3D(StarDistBase):
 
     def train(self, X, Y, validation_data, classes='auto', augmenter=None, seed=None, epochs=None, steps_per_epoch=None, workers=1):
         """Train the network on the device (reference signature; see models/train.py and DESIGN.md 4.2).  Returns a
-        History whose .history holds loss, prob_loss, dist_loss, val_loss, val_prob_loss, val_dist_loss and lr per epoch.
+        History whose .history holds loss, prob_loss, dist_loss, val_loss, val_prob_loss, val_dist_loss and lr per epoch,
+        and prob_class_loss / val_prob_class_loss for multi-class models.
         X, Y and the two of validation_data are lists, tuples or arrays of images, or lazy sequences (len() and
-        __getitem__ returning arrays) read batch by batch (models/data.py).
+        __getitem__ returning arrays) read batch by batch (models/data.py).  For multi-class models `classes` and the
+        optional third entry of validation_data are per-image class ids or label -> class dicts, or 'auto' (n_classes = 1).
         `workers` is accepted for compatibility (batches are made on the device); `train_tensorboard` is ignored."""
         from .train import train
         return train(self, X, Y, validation_data, classes=classes, augmenter=augmenter, seed=seed, epochs=epochs,

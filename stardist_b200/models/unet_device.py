@@ -47,8 +47,9 @@ class UNetDeviceND:
                                 1 if self.nd == 2 else 3, 1 if relu else 0, L.ptr(out), L.stream_ptr()))
         return out
 
-    def _class_branch(self, base):
-        """prob_class [N,...,n_classes+1] from the backbone output `base` (fp32, channels last), or None"""
+    def _class_branch(self, base, keep=False):
+        """prob_class [N,...,n_classes+1] from the backbone output `base` (fp32, channels last), or None.  keep=True stores
+        self.saved_class = (base, the prob_class layer's input, prob_class) for the backward pass."""
         if self.config.n_classes is None:
             return None
         lib = L.load()
@@ -62,6 +63,8 @@ class UNetDeviceND:
         npix = int(np.prod(x.shape[:-1]))
         out = torch.empty(tuple(x.shape[:-1]) + (C,), dtype=torch.float32, device=x.device)
         L.check(lib.sdb_class_head(L.ptr(x), npix, cf, L.ptr(wc.reshape(cf, C).contiguous()), L.ptr(bc), C, L.ptr(out), L.stream_ptr()))
+        if keep:
+            self.saved_class = (base, x, out)
         return out
 
     def _pool(self, x, pool):
@@ -76,7 +79,8 @@ class UNetDeviceND:
     def forward(self, x, keep=False):
         """x: float32 [N,(D,)H,W,Cin] on the device -> (prob [N,...], dist [N,...,R]).
         keep=True stores in self.saved, per entry of self.layers, what the backward pass reads: for a convolution its
-        inputs (x, x_lo, up) and its output y, for a pooling its input x; self.saved_feat is the heads' input."""
+        inputs (x, x_lo, up) and its output y, for a pooling its input x; self.saved_feat is the heads' input and, for
+        multi-class models, self.saved_class the class branch's (see _class_branch)."""
         lib = L.load()
         assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
         skips = {}
@@ -117,7 +121,7 @@ class UNetDeviceND:
         dist = torch.empty(tuple(feat.shape[:-1]) + (R,), dtype=torch.float32, device=x.device)
         L.check(lib.sdb_heads_2d(L.ptr(feat), npix, cf, L.ptr(wp), L.ptr(bp), L.ptr(wd), L.ptr(bd), R,
                                 L.ptr(prob), L.ptr(dist), L.stream_ptr()))
-        self.prob_class = self._class_branch(feat if base is None else base)
+        self.prob_class = self._class_branch(feat if base is None else base, keep=keep)
         return prob, dist
 
 
