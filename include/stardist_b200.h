@@ -295,6 +295,23 @@ int sdb_class_head(const float* d_feat, long long npix, int cfeat, const float* 
                    sdb_stream_t stream);
 int sdb_merge_split(const void* d_hi, const void* d_lo, long long n, float* d_out, sdb_stream_t stream);
 
+/* Any layer shape (csrc/unet_any.cu), for the models outside the default architecture family.  `act` is an activation
+ * id: 0 linear, 1 relu, 2 elu, 3 selu, 4 tanh, 5 sigmoid, 6 softplus, 7 softsign, 8 exponential, 9 swish, 10 gelu.
+ * sdb_conv_any_nd: tiled convolution, NDHWC fp32 (2-D: d = kz = sz = 1), Keras kernels (kz,ky,kx,Cin,Cout) with extents
+ * 1..7, strides 1 or 2 under TensorFlow's padding='same' (out = ceil(in / s), pad_before = pad_total / 2), output
+ * [n, ceil(d/sz), ceil(h/sy), ceil(w/sx), cout] = act(conv + bias).  Input channels are [upsample(in_lo), in] when
+ * cin_lo > 0 (stride 1 only; (uz,uy,ux) nearest up-sampling factors, (d,h,w) the skip's size).
+ * sdb_heads_any: the 1^d heads of sdb_heads_2d for any cfeat >= 1 and 1 <= n_rays <= 256.
+ * sdb_maxpool_any_nd: sdb_maxpool_nd for any c.  sdb_add_act_any: out = act(a + b). */
+int sdb_conv_any_nd(const float* d_in, const float* d_in_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                    int uz, int uy, int ux, const float* d_weight, const float* d_bias, int cout,
+                    int kz, int ky, int kx, int sz, int sy, int sx, int act, float* d_out, sdb_stream_t stream);
+int sdb_heads_any(const float* d_feat, long long npix, int cfeat, const float* d_wp, const float* d_bp,
+                  const float* d_wd, const float* d_bd, int n_rays, float* d_prob, float* d_dist, sdb_stream_t stream);
+int sdb_maxpool_any_nd(const float* d_in, int n, int d, int h, int w, int c, int pz, int py, int px, float* d_out,
+                       sdb_stream_t stream);
+int sdb_add_act_any(const float* d_a, const float* d_b, long long n, int act, float* d_out, sdb_stream_t stream);
+
 /* 1x1 heads: prob = sigmoid(x.Wp+bp) [npix], dist = x.Wd+bd [npix*n_rays] */
 int sdb_heads_2d(const float* d_feat, long long npix, int cfeat, const float* d_wp, const float* d_bp,
                  const float* d_wd, const float* d_bd, int n_rays, float* d_prob, float* d_dist,

@@ -59,6 +59,14 @@ def _declare(lib):
     lib.sdb_class_head.restype = c_int
     lib.sdb_merge_split.argtypes = [P, P, c_longlong, P, P]
     lib.sdb_merge_split.restype = c_int
+    lib.sdb_conv_any_nd.argtypes = [P, P] + [c_int] * 9 + [P, P] + [c_int] * 8 + [P, P]
+    lib.sdb_conv_any_nd.restype = c_int
+    lib.sdb_heads_any.argtypes = [P, c_longlong, c_int, P, P, P, P, c_int, P, P, P]
+    lib.sdb_heads_any.restype = c_int
+    lib.sdb_maxpool_any_nd.argtypes = [P] + [c_int] * 8 + [P, P]
+    lib.sdb_maxpool_any_nd.restype = c_int
+    lib.sdb_add_act_any.argtypes = [P, P, c_longlong, c_int, P, P]
+    lib.sdb_add_act_any.restype = c_int
     lib.sdb_conv_wgrad_workspace.argtypes = [c_longlong, c_int, c_int, c_int]
     lib.sdb_conv_wgrad_workspace.restype = c_longlong
     lib.sdb_conv_wgrad_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, P, c_longlong, P, P, P]

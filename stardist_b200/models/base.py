@@ -874,11 +874,16 @@ class StarDistBase:
         return tuple(n_tiles)
 
     # ------------------------------------------------------------------ misc
-    def _compute_receptive_field(self, img_size=None):
-        """base.py:1068-1098: empirical receptive field from the response to a unit impulse"""
+    def _compute_receptive_field(self, img_size=None, _grow=None):
+        """base.py:1068-1098: empirical receptive field from the response to a unit impulse.  With kernels larger than 3 the
+        receptive field can exceed half of the reference's default probe (a 5x5 U-Net of depth 2 reaches 94 pixels), which
+        would clip it and make n_tiles overlaps too small; for those models the default probe doubles along every axis the
+        response reaches the border of, until it does not (3^d models keep the reference's probe)."""
         from scipy.ndimage import zoom
         if img_size is None:
             img_size = tuple(g * (128 if self.config.n_dim == 2 else 64) for g in self.config.grid)
+            ks = self.config.resnet_kernel_size if getattr(self.config, 'backbone', 'unet') == 'resnet' else self.config.unet_kernel_size
+            _grow = max(int(k) for k in ks) > 3
         if np.isscalar(img_size):
             img_size = (img_size,) * self.config.n_dim
         img_size = tuple(img_size)
@@ -897,7 +902,10 @@ class StarDistBase:
         ind = np.where(np.abs(y - y0) > 0)
         if any(len(i) == 0 for i in ind):
             untrained = type(self)(self.config, name=None, basedir=None)
-            return untrained._compute_receptive_field(img_size=img_size)
+            return untrained._compute_receptive_field(img_size=img_size, _grow=_grow)
+        touch = [np.min(i) == 0 or np.max(i) == s - 1 for i, s in zip(ind, img_size)]
+        if _grow and any(touch) and max(img_size) < 4096:
+            return self._compute_receptive_field(img_size=tuple(2 * s if t else s for s, t in zip(img_size, touch)), _grow=True)
         return [(m - np.min(i), np.max(i) - m) for (m, i) in zip(mid, ind)]
 
     def _axes_tile_overlap(self, query_axes):

@@ -14,6 +14,7 @@ from .base import StarDistBase
 from .config import Config2D
 import os
 from .unet_device import UNetDevice2D, UNetDevice2DTC
+from .weights import unet_layers
 
 
 class StarDist2D(StarDistBase):
@@ -35,7 +36,9 @@ class StarDist2D(StarDistBase):
         # default: tcgen05 tensor-core path; STARDIST_B200_UNET=simt selects the exact-fp32 CUDA-core
         # kernels (also used automatically for layer shapes the tensor-core kernel does not cover)
         mode = os.environ.get("STARDIST_B200_UNET", "tc").lower()
-        if mode != "simt" and UNetDevice2DTC.supported(self.config):
+        # the tensor-core convolutions apply ReLU or nothing; other activations run on the CUDA-core kernels
+        tc_acts = all(l['act'] in ('relu', 'linear') for l in unet_layers(self.config) if l['kind'] == 'conv')
+        if mode != "simt" and tc_acts and UNetDevice2DTC.supported(self.config):
             return UNetDevice2DTC(self.config, self.weights)
         return UNetDevice2D(self.config, self.weights)
 

@@ -12,39 +12,104 @@ from .. import _lib as L
 from .weights import unet_layers, resnet_layers
 
 
+# Keras activation name -> activation id of the csrc/unet_any.cu kernels (0 and 1 are also the `relu` flag of unet_simt.cu)
+ACTIVATIONS = {'linear': 0, 'relu': 1, 'elu': 2, 'selu': 3, 'tanh': 4, 'sigmoid': 5, 'softplus': 6, 'softsign': 7,
+               'exponential': 8, 'swish': 9, 'gelu': 10}
+
+
+def act_id(name):
+    """activation id of a Keras activation name; NotImplementedError naming it for any other (e.g. 'hard_sigmoid', whose
+    definition changed between Keras versions)"""
+    if name not in ACTIVATIONS:
+        raise NotImplementedError("activation %r is not supported (supported: %s)" % (name, ", ".join(ACTIVATIONS)))
+    return ACTIVATIONS[name]
+
+
+def check_activations(layers):
+    """act_id of every activation of a layer list, so that an unsupported one raises before anything touches the device"""
+    for l in layers:
+        if l['kind'] in ('conv', 'conv_class', 'block_end'):
+            act_id(l['act'])
+
+
+# One predicate per unet_simt.cu kernel: the layers it accepts run on it, every other layer on csrc/unet_any.cu.
+def conv3_accepts(nd, k, stride, cin_skip, cin_lo, cout, act):
+    """sdb_conv3_nd: 3^d kernels at stride 1 with ReLU or linear; its stem variant takes cin <= 4 without an up-sampled
+    source and cout 32 or 64, its tiled variant input channels in multiples of 8 and output channels in multiples of 32"""
+    if tuple(k) != (3,) * nd or tuple(stride) != (1,) * nd or act not in ('relu', 'linear'):
+        return False
+    if cin_lo == 0 and cin_skip <= 4:
+        return cout in (32, 64)
+    return cin_skip % 8 == 0 and cin_lo % 8 == 0 and cout % 32 == 0
+
+
+def conv_generic_accepts(act):
+    """sdb_conv_generic_nd: any kernel extent and stride, ReLU or linear"""
+    return act in ('relu', 'linear')
+
+
+def maxpool_accepts(c):
+    """sdb_maxpool_nd: channel counts that are multiples of 4"""
+    return c % 4 == 0
+
+
+def heads_accept(cf, n_rays):
+    """sdb_heads_2d: 128 feature channels, and its weight and output tables within 200 KB of shared memory"""
+    return cf == 128 and (160 * (n_rays + 1) + 32 * 129) * 4 <= 200 * 1024
+
+
+def add_act_accepts(act):
+    """sdb_add_act: ReLU or linear"""
+    return act in ('relu', 'linear')
+
+
 class UNetDeviceND:
-    """exact-fp32 CUDA-core executor (csrc/unet_simt.cu) for 2-D (NHWC) and 3-D (NDHWC) U-Nets"""
+    """exact-fp32 CUDA-core executor for 2-D (NHWC) and 3-D (NDHWC) U-Nets: csrc/unet_simt.cu for the layers its kernels
+    accept (see the *_accepts predicates), csrc/unet_any.cu for every other kernel extent, channel count, feature width and
+    activation"""
 
     def __init__(self, config, weights, device=None):
+        if config.unet_batch_norm:
+            raise NotImplementedError("unet_batch_norm=True is not supported on this path")
+        self.layers = unet_layers(config)
+        check_activations(self.layers)
         L.require_cuda()
         self.config = config
         self.nd = config.n_dim
         self.device = torch.device("cuda") if device is None else torch.device(device)
-        self.layers = unet_layers(config)
+        self._upload(weights)
+
+    def _upload(self, weights):
         self.w = {}
         for name, (k, b) in weights.items():
             self.w[name] = (torch.from_numpy(np.ascontiguousarray(k, dtype=np.float32)).to(self.device),
                             torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)).to(self.device))
-        if config.unet_batch_norm:
-            raise NotImplementedError("unet_batch_norm=True is not supported on this path")
-        if tuple(config.unet_kernel_size) != (3,) * self.nd:
-            raise NotImplementedError("only 3^d kernels are supported")
 
     @staticmethod
     def _dhw(x):
         return (1,) + tuple(x.shape[1:3]) if x.dim() == 4 else tuple(x.shape[1:4])
 
-    def _conv(self, x, x_lo, name, relu, up):
+    def _conv(self, x, x_lo, name, act, up, stride=None):
+        """act(conv(x) + bias) with 'same' padding; the input channels are [upsample(x_lo), x] when x_lo is given"""
         lib = L.load()
         k, b = self.w[name]
         n = x.shape[0]; d, h, w = self._dhw(x); c_skip = x.shape[-1]
         c_lo = 0 if x_lo is None else x_lo.shape[-1]
         cout = k.shape[-1]
         assert k.shape[-2] == c_skip + c_lo, (name, k.shape, c_skip, c_lo)
-        out = torch.empty(tuple(x.shape[:-1]) + (cout,), dtype=torch.float32, device=x.device)
+        ks = tuple(k.shape[:-2])
+        stride = (1,) * self.nd if stride is None else tuple(stride)
         uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
-        L.check(lib.sdb_conv3_nd(L.ptr(x), L.ptr(x_lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), L.ptr(k), L.ptr(b), cout,
-                                1 if self.nd == 2 else 3, 1 if relu else 0, L.ptr(out), L.stream_ptr()))
+        if conv3_accepts(self.nd, ks, stride, c_skip, c_lo, cout, act):
+            out = torch.empty(tuple(x.shape[:-1]) + (cout,), dtype=torch.float32, device=x.device)
+            L.check(lib.sdb_conv3_nd(L.ptr(x), L.ptr(x_lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), L.ptr(k), L.ptr(b), cout,
+                                    1 if self.nd == 2 else 3, 1 if act == 'relu' else 0, L.ptr(out), L.stream_ptr()))
+            return out
+        (kz, ky, kx), (sz, sy, sx) = ((1,) + ks, (1,) + stride) if self.nd == 2 else (ks, stride)
+        osp = tuple(-(-s // t) for s, t in zip(x.shape[1:-1], stride))
+        out = torch.empty((n,) + osp + (cout,), dtype=torch.float32, device=x.device)
+        L.check(lib.sdb_conv_any_nd(L.ptr(x), L.ptr(x_lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), L.ptr(k), L.ptr(b), cout,
+                                   kz, ky, kx, sz, sy, sx, act_id(act), L.ptr(out), L.stream_ptr()))
         return out
 
     def _class_branch(self, base, keep=False):
@@ -55,9 +120,8 @@ class UNetDeviceND:
         lib = L.load()
         x = base
         if 'features_class' in self.w:
-            k = self.w['features_class'][0]
             act = self.config.unet_activation if getattr(self.config, 'backbone', 'unet') == 'unet' else self.config.resnet_activation
-            x = self._conv(base, None, 'features_class', act == 'relu', (1,) * self.nd)
+            x = self._conv(base, None, 'features_class', act, (1,) * self.nd)
         wc, bc = self.w['prob_class']
         C = int(wc.shape[-1]); cf = int(x.shape[-1])
         npix = int(np.prod(x.shape[:-1]))
@@ -73,15 +137,27 @@ class UNetDeviceND:
         pz, py, px = ((1,) + tuple(pool)) if len(pool) == 2 else tuple(pool)
         osp = (h // py, w // px) if self.nd == 2 else (d // pz, h // py, w // px)
         out = torch.empty((n,) + osp + (c,), dtype=torch.float32, device=x.device)
-        L.check(lib.sdb_maxpool_nd(L.ptr(x), n, d, h, w, c, int(pz), int(py), int(px), L.ptr(out), L.stream_ptr()))
+        fn = lib.sdb_maxpool_nd if maxpool_accepts(c) else lib.sdb_maxpool_any_nd
+        L.check(fn(L.ptr(x), n, d, h, w, c, int(pz), int(py), int(px), L.ptr(out), L.stream_ptr()))
         return out
+
+    def _heads(self, feat):
+        lib = L.load()
+        cf = feat.shape[-1]
+        npix = int(np.prod(feat.shape[:-1]))
+        R = self.config.n_rays
+        (wp, bp), (wd, bd) = self.w['prob'], self.w['dist']
+        prob = torch.empty(tuple(feat.shape[:-1]), dtype=torch.float32, device=feat.device)
+        dist = torch.empty(tuple(feat.shape[:-1]) + (R,), dtype=torch.float32, device=feat.device)
+        fn = lib.sdb_heads_2d if heads_accept(cf, R) else lib.sdb_heads_any
+        L.check(fn(L.ptr(feat), npix, cf, L.ptr(wp), L.ptr(bp), L.ptr(wd), L.ptr(bd), R, L.ptr(prob), L.ptr(dist), L.stream_ptr()))
+        return prob, dist
 
     def forward(self, x, keep=False):
         """x: float32 [N,(D,)H,W,Cin] on the device -> (prob [N,...], dist [N,...,R]).
         keep=True stores in self.saved, per entry of self.layers, what the backward pass reads: for a convolution its
         inputs (x, x_lo, up) and its output y, for a pooling its input x; self.saved_feat is the heads' input and, for
         multi-class models, self.saved_class the class branch's (see _class_branch)."""
-        lib = L.load()
         assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
         skips = {}
         lo, up = None, (1,) * self.nd
@@ -90,11 +166,8 @@ class UNetDeviceND:
         for i, l in enumerate(self.layers):
             kind = l['kind']
             if kind == 'conv':
-                act = l['act']
-                if act not in ('relu', 'linear'):
-                    raise NotImplementedError("activation %s" % act)
                 if l['name'] == 'features': base = x
-                y = self._conv(x, lo, l['name'], act == 'relu', up)
+                y = self._conv(x, lo, l['name'], l['act'], up)
                 if keep:
                     saved[i] = dict(x=x, lo=lo, up=up, y=y)
                 x = y
@@ -113,14 +186,7 @@ class UNetDeviceND:
         feat = x
         if keep:
             self.saved, self.saved_feat = saved, feat
-        cf = feat.shape[-1]
-        npix = int(np.prod(feat.shape[:-1]))
-        R = self.config.n_rays
-        (wp, bp), (wd, bd) = self.w['prob'], self.w['dist']
-        prob = torch.empty(tuple(feat.shape[:-1]), dtype=torch.float32, device=x.device)
-        dist = torch.empty(tuple(feat.shape[:-1]) + (R,), dtype=torch.float32, device=x.device)
-        L.check(lib.sdb_heads_2d(L.ptr(feat), npix, cf, L.ptr(wp), L.ptr(bp), L.ptr(wd), L.ptr(bd), R,
-                                L.ptr(prob), L.ptr(dist), L.stream_ptr()))
+        prob, dist = self._heads(feat)
         self.prob_class = self._class_branch(feat if base is None else base, keep=keep)
         return prob, dist
 
@@ -132,34 +198,34 @@ class ResNetDeviceND(UNetDeviceND):
     """3-D ResNet backbone (stardist/models/model3d.py:402-447, csbdeep resnet_block) on the fp32 CUDA-core kernels:
     the stride-1 3^3 convolutions run on the tiled kernel of the U-Net path (sdb_conv3_nd), the 7^3 stem, the strided
     3^3 convolution that opens a pooling block and the strided 1^3 shortcut projection on the generic kernel
-    (sdb_conv_generic_nd, TensorFlow 'same' padding), the residual sum on sdb_add_act."""
+    (sdb_conv_generic_nd, TensorFlow 'same' padding), the residual sum on sdb_add_act.  Layers none of these accept
+    (activations other than ReLU / linear, channel counts sdb_conv3_nd does not take) run on csrc/unet_any.cu."""
 
     def __init__(self, config, weights, device=None):
+        self.layers = resnet_layers(config)
+        check_activations(self.layers)
         L.require_cuda()
         self.config = config
         self.nd = config.n_dim
         self.device = torch.device("cuda") if device is None else torch.device(device)
-        self.layers = resnet_layers(config)
-        self.w = {}
-        for name, (k, b) in weights.items():
-            self.w[name] = (torch.from_numpy(np.ascontiguousarray(k, dtype=np.float32)).to(self.device),
-                            torch.from_numpy(np.ascontiguousarray(b, dtype=np.float32)).to(self.device))
+        self._upload(weights)
 
-    def _conv_any(self, x, l):
+    def _conv_layer(self, x, l):
         lib = L.load()
         k, b = self.w[l['name']]
-        relu = l['act'] == 'relu'
-        if l['act'] not in ('relu', 'linear'):
-            raise NotImplementedError("activation %s" % l['act'])
+        act = l['act']
         if tuple(l['k']) == (3, 3, 3) and tuple(l['stride']) == (1, 1, 1) and l['cin'] > 4:
-            return self._conv(x, None, l['name'], relu, (1, 1, 1))
-        n, d, h, w, cin = x.shape
-        kz, ky, kx = l['k']; sz, sy, sx = l['stride']
-        cout = k.shape[-1]
-        out = torch.empty((n, -(-d // sz), -(-h // sy), -(-w // sx), cout), dtype=torch.float32, device=x.device)
-        L.check(lib.sdb_conv_generic_nd(L.ptr(x), n, d, h, w, cin, L.ptr(k), L.ptr(b), cout, kz, ky, kx, sz, sy, sx,
-                                       1 if relu else 0, L.ptr(out), L.stream_ptr()))
-        return out
+            if conv3_accepts(3, l['k'], l['stride'], l['cin'], 0, l['cout'], act):
+                return self._conv(x, None, l['name'], act, (1, 1, 1))
+        elif conv_generic_accepts(act):
+            n, d, h, w, cin = x.shape
+            kz, ky, kx = l['k']; sz, sy, sx = l['stride']
+            cout = k.shape[-1]
+            out = torch.empty((n, -(-d // sz), -(-h // sy), -(-w // sx), cout), dtype=torch.float32, device=x.device)
+            L.check(lib.sdb_conv_generic_nd(L.ptr(x), n, d, h, w, cin, L.ptr(k), L.ptr(b), cout, kz, ky, kx, sz, sy, sx,
+                                           1 if act == 'relu' else 0, L.ptr(out), L.stream_ptr()))
+            return out
+        return self._conv(x, None, l['name'], act, (1, 1, 1), stride=l['stride'])
 
     def forward(self, x):
         lib = L.load()
@@ -171,26 +237,22 @@ class ResNetDeviceND(UNetDeviceND):
                 block_in, shortcut = x, None
             elif kind == 'conv':
                 if l['name'] == 'features': base = x
-                y = self._conv_any(block_in if l['src'] == 'block_in' else x, l)
+                y = self._conv_layer(block_in if l['src'] == 'block_in' else x, l)
                 if l['dst'] == 'shortcut': shortcut = y
                 else: x = y
             elif kind == 'block_end':
                 s = block_in if shortcut is None else shortcut
                 assert s.shape == x.shape
                 out = torch.empty_like(x)
-                L.check(lib.sdb_add_act(L.ptr(s), L.ptr(x), x.numel(), 1 if l['act'] == 'relu' else 0, L.ptr(out), L.stream_ptr()))
+                if add_act_accepts(l['act']):
+                    L.check(lib.sdb_add_act(L.ptr(s), L.ptr(x), x.numel(), 1 if l['act'] == 'relu' else 0, L.ptr(out), L.stream_ptr()))
+                else:
+                    L.check(lib.sdb_add_act_any(L.ptr(s), L.ptr(x), x.numel(), act_id(l['act']), L.ptr(out), L.stream_ptr()))
                 x, block_in, shortcut = out, None, None
             elif kind == 'head':
                 break
         feat = x
-        cf = feat.shape[-1]
-        npix = int(np.prod(feat.shape[:-1]))
-        R = self.config.n_rays
-        (wp, bp), (wd, bd) = self.w['prob'], self.w['dist']
-        prob = torch.empty(tuple(feat.shape[:-1]), dtype=torch.float32, device=x.device)
-        dist = torch.empty(tuple(feat.shape[:-1]) + (R,), dtype=torch.float32, device=x.device)
-        L.check(lib.sdb_heads_2d(L.ptr(feat), npix, cf, L.ptr(wp), L.ptr(bp), L.ptr(wd), L.ptr(bd), R,
-                                L.ptr(prob), L.ptr(dist), L.stream_ptr()))
+        prob, dist = self._heads(feat)
         self.prob_class = self._class_branch(feat if base is None else base)
         return prob, dist
 
@@ -440,7 +502,7 @@ class UNetDevice3DTC:
                 ent = self.w[l['name']]
                 cout = ent['k'].shape[-1]
                 if first:
-                    y = self._simt._conv(x, None, l['name'], bool(relu), (1, 1, 1))          # [1,D,H,W,cout] fp32
+                    y = self._simt._conv(x, None, l['name'], l['act'], (1, 1, 1))          # [1,D,H,W,cout] fp32
                     out = torch.empty((2,) + tuple(y.shape[1:]), dtype=torch.float16, device=x.device)
                     L.check(lib.sdb_split_f32(L.ptr(y), y.numel(), L.ptr(out[0]), L.ptr(out[1]), st))
                     first = False
