@@ -311,6 +311,15 @@ int sdb_heads_any(const float* d_feat, long long npix, int cfeat, const float* d
 int sdb_maxpool_any_nd(const float* d_in, int n, int d, int h, int w, int c, int pz, int py, int px, float* d_out,
                        sdb_stream_t stream);
 int sdb_add_act_any(const float* d_a, const float* d_b, long long n, int act, float* d_out, sdb_stream_t stream);
+/* sdb_act_any: y = act(z) elementwise (y may be z), the epilogue of sdb_conv_any_nd as a separate pass: a convolution run
+ * linear and then this gives the fused result bit for bit.  sdb_act_backward: g *= act'(z) in place, z the pre-activation;
+ * relu zeroes g where z <= 0.  sdb_conv_dgrad_any_nd: input gradient of a stride-1 'same' convolution with kernel extents
+ * (kz,ky,kx) in 1..7, any cin and cout: dx [n,d,h,w,cin] from dy [n,d,h,w,cout] and wf (kz,ky,kx,cout,cin), the kernel
+ * flipped by sdb_conv_flip_weights; a decoder layer's dx is d[upsample(x_lo), skip], split by sdb_decoder_split. */
+int sdb_act_any(const float* d_z, long long n, int act, float* d_y, sdb_stream_t stream);
+int sdb_act_backward(float* d_g, const float* d_z, long long n, int act, sdb_stream_t stream);
+int sdb_conv_dgrad_any_nd(const float* d_dy, int n, int d, int h, int w, int cout, const float* d_wf, int cin,
+                          int kz, int ky, int kx, float* d_dx, sdb_stream_t stream);
 
 /* 1x1 heads: prob = sigmoid(x.Wp+bp) [npix], dist = x.Wd+bd [npix*n_rays] */
 int sdb_heads_2d(const float* d_feat, long long npix, int cfeat, const float* d_wp, const float* d_bp,
@@ -415,8 +424,14 @@ long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin, int cout);
 int sdb_conv_wgrad_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
                       int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
                       long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
-/* wf (k..., cout, cin) = w (k..., cin, cout) flipped along every spatial axis: the input gradient of a stride-1 'same'
- * convolution is sdb_conv3_nd of dy with wf, zero bias, no ReLU */
+/* the same for any kernel extents (kz,ky,kx) in 1..7 at stride 1, TensorFlow 'same' front offsets (k - 1) / 2; the
+ * workspace is sdb_conv_wgrad_workspace(n*d*h*w, kz*ky*kx, cin_skip + cin_lo, cout) floats */
+int sdb_conv_wgrad_any_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                          int uz, int uy, int ux, int kz, int ky, int kx, const float* d_dy, int ldy, int cout, float* d_work,
+                          long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
+/* wf (k..., cout, cin) = w (k..., cin, cout) flipped along every spatial axis (taps = the kernel's box volume): the input
+ * gradient of a stride-1 3^d 'same' convolution is sdb_conv3_nd of dy with wf, zero bias, no ReLU (sdb_conv_dgrad_any_nd
+ * for other extents) */
 int sdb_conv_flip_weights(const float* d_w, int taps, int cin, int cout, float* d_wf, sdb_stream_t stream);
 /* gradient of [upsample(x_lo), skip] -> d x_lo (block sums, the backward of nearest up-sampling) and d skip (overwritten) */
 int sdb_decoder_split(const float* d_dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy, int ux,

@@ -71,6 +71,14 @@ def _declare(lib):
     lib.sdb_conv_wgrad_workspace.restype = c_longlong
     lib.sdb_conv_wgrad_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, P, c_longlong, P, P, P]
     lib.sdb_conv_wgrad_nd.restype = c_int
+    lib.sdb_conv_wgrad_any_nd.argtypes = [P, P] + [c_int] * 12 + [P, c_int, c_int, P, c_longlong, P, P, P]
+    lib.sdb_conv_wgrad_any_nd.restype = c_int
+    lib.sdb_conv_dgrad_any_nd.argtypes = [P] + [c_int] * 5 + [P] + [c_int] * 4 + [P, P]
+    lib.sdb_conv_dgrad_any_nd.restype = c_int
+    lib.sdb_act_any.argtypes = [P, c_longlong, c_int, P, P]
+    lib.sdb_act_any.restype = c_int
+    lib.sdb_act_backward.argtypes = [P, P, c_longlong, c_int, P]
+    lib.sdb_act_backward.restype = c_int
     lib.sdb_conv_flip_weights.argtypes = [P, c_int, c_int, c_int, P, P]
     lib.sdb_conv_flip_weights.restype = c_int
     lib.sdb_decoder_split.argtypes = [P] + [c_int] * 9 + [P, P, P]

@@ -4,12 +4,14 @@
 // of 8 / 32, 128 feature channels).  These cover what a model folder of the reference may hold beyond that: kernel extents
 // 1..7 per axis (odd or even), strides 1 / 2 under TensorFlow's padding='same' rule, any channel count, any feature width,
 // and the Keras activations of the table below.  The executors (models/unet_device.py) use them only for the layers the
-// unet_simt.cu kernels do not accept.
+// unet_simt.cu kernels do not accept.  For training the same layers, the tiled convolution also serves as the input
+// gradient (sdb_conv_dgrad_any_nd), and sdb_act_any / sdb_act_backward split the activation off the convolution.
 //
 // Activation ids (the `act` argument; 0 and 1 match the `relu` flag of the older kernels):
 //   0 linear, 1 relu, 2 elu, 3 selu, 4 tanh, 5 sigmoid, 6 softplus, 7 softsign, 8 exponential, 9 swish, 10 gelu
 #include <cmath>
 #include <algorithm>
+#include <string>
 #include "common.cuh"
 #include "../../include/stardist_b200.h"
 
@@ -41,6 +43,33 @@ __device__ __forceinline__ float act_apply(int act, float x) {
     case 8: return expf(x);
     case 9: return x / (1.f + expf(-x));
     default: return 0.5f * x * erfcf(x * -0.707106781186547524f);
+  }
+}
+
+// act'(z) of the table above in float32 forms without cancellation at either end: elu / selu use exp(z) for z <= 0 (which
+// expm1(z) + 1 would lose to cancellation once expm1(z) rounds to -1), tanh' = 4u / (1 + u)^2 with u = exp(-2|z|) and
+// sigmoid' = u / (1 + u)^2 with u = exp(-|z|) (no 1 - t^2 or s(1 - s) near saturation), softplus' = sigmoid(z) from the
+// same u (the derivative of log(1 + e^z); the thresholds of act_apply only choose how that function is evaluated, and
+// their pieces differ from it by less than one float32 rounding), swish' = s (1 + z (1 - s)) with s and 1 - s both from
+// u, gelu' = 0.5 erfc(-z / sqrt 2) + z exp(-z^2 / 2) / sqrt(2 pi).  relu' is 1 for z > 0 and 0 otherwise (TensorFlow's
+// ReluGrad).
+__device__ __forceinline__ float act_grad(int act, float z) {
+  switch (act) {
+    case 0: return 1.f;
+    case 1: return z > 0.f ? 1.f : 0.f;
+    case 2: return z > 0.f ? 1.f : expf(z);
+    case 3: return z > 0.f ? 1.05070098735548049342f : 1.75809934084737685994f * expf(z);
+    case 4: { const float u = expf(-2.f * fabsf(z)), q = 1.f + u; return 4.f * u / (q * q); }
+    case 5: { const float u = expf(-fabsf(z)), q = 1.f + u; return u / (q * q); }
+    case 6: { const float u = expf(-fabsf(z)); return (z >= 0.f ? 1.f : u) / (1.f + u); }
+    case 7: { const float q = 1.f + fabsf(z); return 1.f / (q * q); }
+    case 8: return expf(z);
+    case 9: {
+      const float u = expf(-fabsf(z)), r = 1.f / (1.f + u);
+      const float s = z >= 0.f ? r : u * r, sc = z >= 0.f ? u * r : r;      // sigmoid(z), 1 - sigmoid(z)
+      return s * (1.f + z * sc);
+    }
+    default: return 0.5f * erfcf(z * -0.707106781186547524f) + z * 0.398942280401432678f * expf(-0.5f * z * z);
   }
 }
 
@@ -133,7 +162,7 @@ k_conv_any(const float* __restrict__ in_skip, const float* __restrict__ in_lo, c
   if (oy >= P.oh || co0 >= P.cout) return;
   float bb[8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) bb[j] = (co0 + j < P.cout) ? bias[co0 + j] : 0.f;
+  for (int j = 0; j < 8; ++j) bb[j] = (bias != nullptr && co0 + j < P.cout) ? bias[co0 + j] : 0.f;
   const bool vec = (P.cout % 4 == 0) && (co0 + 8 <= P.cout);
   float* orow = out + ((((size_t)img * P.od + zo) * P.oh + oy) * (size_t)P.ow) * P.cout + co0;
 #pragma unroll
@@ -237,6 +266,20 @@ __global__ void k_add_act_any(const float* __restrict__ a, const float* __restri
     out[e] = act_apply(act, a[e] + b[e]);
 }
 
+__global__ void k_act_any(const float* __restrict__ z, long long n, int act, float* __restrict__ y) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x)
+    y[e] = act_apply(act, z[e]);
+}
+
+// g *= act'(z); relu zeroes g where z <= 0 (also an infinite g), like sdb_relu_backward
+__global__ void k_act_backward(float* __restrict__ g, const float* __restrict__ z, long long n, int act) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+    const float v = z[e];
+    if (act == 1) { if (!(v > 0.f)) g[e] = 0.f; }
+    else g[e] *= act_grad(act, v);
+  }
+}
+
 template <int COUT_T, int SX>
 int launch_conv(dim3 grid, size_t smem, cudaStream_t st, const float* in, const float* lo, const float* w, const float* b,
                 const ConvAny& P, float* out) {
@@ -244,6 +287,25 @@ int launch_conv(dim3 grid, size_t smem, cudaStream_t st, const float* in, const 
   if (!attr) { SDB_CUDA(cudaFuncSetAttribute(k_conv_any<COUT_T, SX>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
   SDB_LAUNCH((k_conv_any<COUT_T, SX>), grid, COUT_T * 4, smem, st, in, lo, w, b, P, out);
   return 0;
+}
+
+// launches k_conv_any for P with its pads (pz, py, px) already set; the sizes, kernel and channels of P are checked by the caller
+int run_conv_any(const char* who, ConvAny& P, int n, const float* d_in, const float* d_in_lo, const float* d_weight, const float* d_bias,
+                 float* d_out, cudaStream_t st) {
+  P.rows = (kTH - 1) * P.sy + P.ky; P.cols = (kTW - 1) * P.sx + P.kx;
+  P.plane = (P.rows * P.cols) | 1;                  // odd: the channel-major halo stores avoid bank conflicts
+  P.tiles_x = cdiv(P.ow, kTW);
+  const int cout_t = P.cout > 32 ? 64 : 32;
+  const long long gx = (long long)P.tiles_x * cdiv(P.oh, kTH), gy = cdiv(P.cout, cout_t), gz = (long long)n * P.od;
+  if (gx > 0x7fffffffLL || gy > 65535 || gz > 65535) { sdb::set_error(std::string(who) + ": grid too large"); return 1; }
+  const size_t smem = (size_t)(kCK * P.plane + P.ky * P.kx * kCK * cout_t) * sizeof(float);
+  dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)gz);
+  if (cout_t == 64) {
+    if (P.sx == 1) return launch_conv<64, 1>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
+    return launch_conv<64, 2>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
+  }
+  if (P.sx == 1) return launch_conv<32, 1>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
+  return launch_conv<32, 2>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
 }
 
 }  // namespace
@@ -273,20 +335,7 @@ extern "C" int sdb_conv_any_nd(const float* d_in, const float* d_in_lo, int n, i
   P.pz = std::max((P.od - 1) * sz + kz - d, 0) / 2;
   P.py = std::max((P.oh - 1) * sy + ky - h, 0) / 2;
   P.px = std::max((P.ow - 1) * sx + kx - w, 0) / 2;
-  P.rows = (kTH - 1) * sy + ky; P.cols = (kTW - 1) * sx + kx;
-  P.plane = (P.rows * P.cols) | 1;                  // odd: the channel-major halo stores avoid bank conflicts
-  P.tiles_x = cdiv(P.ow, kTW);
-  const int cout_t = cout > 32 ? 64 : 32;
-  const long long gx = (long long)P.tiles_x * cdiv(P.oh, kTH), gy = cdiv(cout, cout_t), gz = (long long)n * P.od;
-  if (gx > 0x7fffffffLL || gy > 65535 || gz > 65535) { sdb::set_error("conv_any_nd: grid too large"); return 1; }
-  const size_t smem = (size_t)(kCK * P.plane + ky * kx * kCK * cout_t) * sizeof(float);
-  dim3 grid((unsigned)gx, (unsigned)gy, (unsigned)gz);
-  if (cout_t == 64) {
-    if (sx == 1) return launch_conv<64, 1>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
-    return launch_conv<64, 2>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
-  }
-  if (sx == 1) return launch_conv<32, 1>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
-  return launch_conv<32, 2>(grid, smem, st, d_in, d_in_lo, d_weight, d_bias, P, d_out);
+  return run_conv_any("conv_any_nd", P, n, d_in, d_in_lo, d_weight, d_bias, d_out, st);
 }
 
 extern "C" int sdb_heads_any(const float* d_feat, long long npix, int cfeat, const float* d_wp, const float* d_bp,
@@ -318,5 +367,36 @@ extern "C" int sdb_add_act_any(const float* d_a, const float* d_b, long long n, 
   if (act < 0 || act >= kNumActs) { sdb::set_error("add_act_any: unknown activation id"); return 1; }
   if (n <= 0) return 0;
   SDB_LAUNCH(k_add_act_any, (int)std::min<long long>(cdiv(n, 256LL), 132 * 32), 256, 0, st, d_a, d_b, n, act, d_out);
+  return 0;
+}
+
+// dX of a stride-1 'same' convolution with kernel (kz, ky, kx, cin, cout): the correlation of dY with the flipped kernel
+// wf (kz, ky, kx, cout, cin) of sdb_conv_flip_weights, front offset k - 1 - (k - 1) / 2 per axis (the forward's back
+// padding, which differs from its front padding for even k), zero bias, linear output, on the tiled kernel above
+extern "C" int sdb_conv_dgrad_any_nd(const float* d_dy, int n, int d, int h, int w, int cout, const float* d_wf, int cin,
+                                     int kz, int ky, int kx, float* d_dx, sdb_stream_t stream) {
+  if (n <= 0 || d <= 0 || h <= 0 || w <= 0 || cin < 1 || cout < 1) { sdb::set_error("conv_dgrad_any_nd: bad sizes"); return 1; }
+  if (kz < 1 || kz > 7 || ky < 1 || ky > 7 || kx < 1 || kx > 7) { sdb::set_error("conv_dgrad_any_nd: kernel extents must be in 1..7"); return 1; }
+  ConvAny P;
+  P.d = d; P.h = h; P.w = w; P.c_skip = cout; P.c_lo = 0; P.uz = P.uy = P.ux = 1;
+  P.cout = cin; P.kz = kz; P.ky = ky; P.kx = kx; P.sz = P.sy = P.sx = 1; P.act = 0;
+  P.od = d; P.oh = h; P.ow = w;
+  P.pz = kz - 1 - (kz - 1) / 2; P.py = ky - 1 - (ky - 1) / 2; P.px = kx - 1 - (kx - 1) / 2;
+  return run_conv_any("conv_dgrad_any_nd", P, n, d_dy, nullptr, d_wf, nullptr, d_dx, (cudaStream_t)stream);
+}
+
+extern "C" int sdb_act_any(const float* d_z, long long n, int act, float* d_y, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (act < 0 || act >= kNumActs) { sdb::set_error("act_any: unknown activation id"); return 1; }
+  if (n <= 0) return 0;
+  SDB_LAUNCH(k_act_any, (int)std::min<long long>(cdiv(n, 256LL), 132 * 32), 256, 0, st, d_z, n, act, d_y);
+  return 0;
+}
+
+extern "C" int sdb_act_backward(float* d_g, const float* d_z, long long n, int act, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (act < 0 || act >= kNumActs) { sdb::set_error("act_backward: unknown activation id"); return 1; }
+  if (n <= 0 || act == 0) return 0;
+  SDB_LAUNCH(k_act_backward, (int)std::min<long long>(cdiv(n, 256LL), 132 * 32), 256, 0, st, d_g, d_z, n, act);
   return 0;
 }

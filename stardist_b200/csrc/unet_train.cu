@@ -1,13 +1,15 @@
 // unet_train.cu -- fp32 CUDA-core kernels of the U-Net training step (NHWC / NDHWC): weight gradients of the
 // 3^d / 1^d convolutions, the decoder split, ReLU and max-pool backward, the StarDist loss with its head gradient,
-// the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients and Adam.  The input gradient of the 3^d convolutions is not here: it is the forward
-// kernel of unet_simt.cu (sdb_conv3_nd) run on dY with the spatially flipped, Cin/Cout-transposed kernel written by
-// sdb_conv_flip_weights.
+// the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients and Adam.  The input gradient of the
+// convolutions is not here: it is a forward kernel run on dY with the spatially flipped, Cin/Cout-transposed kernel written by
+// sdb_conv_flip_weights -- sdb_conv3_nd of unet_simt.cu for the 3^d layers it takes, sdb_conv_dgrad_any_nd of unet_any.cu
+// for every other kernel extent and channel count.
 //
 // Determinism: no float atomics anywhere.  Every reduction splits its work into a count of pieces taken from the shape
 // alone, each piece accumulates in a fixed order into its own slot of a workspace, and a second kernel sums the slots
 // in index order.  Gradients, loss values and weights are therefore bit-identical from run to run on the same device.
 #include <math.h>
+#include <string>
 #include <algorithm>
 #include "common.cuh"
 #include "../../include/stardist_b200.h"
@@ -19,8 +21,10 @@ using sdb::cdiv;
 __device__ __forceinline__ long long llmin(long long a, long long b) { return a < b ? a : b; }
 
 // ------------------------------------------------------------------------------------------ weight gradient
-// dW[tap, ci, co] = sum_p x[p + tap, ci] * dy[p, co] and db[co] = sum_p dy[p, co], as one GEMM over the pixels p of the
-// whole batch: row r < taps*Cin is (tap, ci) = (r / Cin, r % Cin), row taps*Cin is a constant 1 (the bias).  The decoder
+// dW[tap, ci, co] = sum_p x[p + tap - pad, ci] * dy[p, co] and db[co] = sum_p dy[p, co], as one GEMM over the pixels p of the
+// whole batch: row r < taps*Cin is (tap, ci) = (r / Cin, r % Cin), tap = (dz, dy, dx) row-major over the (kz, ky, kx) box,
+// row taps*Cin is a constant 1 (the bias).  pad is TensorFlow's 'same' front offset at stride 1, (k - 1) / 2 per axis
+// (k / 2 for odd k, so the 3^d / 1^d path of sdb_conv_wgrad_nd reads what it always read).  The decoder
 // input [upsample(x_lo), skip] is read through the forward loader's address math (channel c < c_lo from x_lo at the
 // up-sampled position).  CTA tile 64 rows x 64 output channels, 16 pixels per K step, 4x4 outputs per thread; split s of
 // the pixel range writes work[s][row][co].
@@ -28,7 +32,7 @@ constexpr int WG_R = 64, WG_C = 64, WG_K = 16;
 
 struct WgradArgs {
   const float* x; const float* x_lo; const float* dy;
-  int n, d, h, w, c_skip, c_lo, uz, uy, ux, kz, kyx, ldy, cout;
+  int n, d, h, w, c_skip, c_lo, uz, uy, ux, kz, ky, kx, pz, py, px, ldy, cout;
   int rows;                 // taps * Cin + 1
   long long npix, per_split;
   float* work;
@@ -39,17 +43,16 @@ __global__ void __launch_bounds__(256) k_conv_wgrad(WgradArgs A) {
   __shared__ __align__(16) float sD[WG_K][WG_C];
   __shared__ int sRow[WG_R][5];          // dz, dy, dx, channel, kind (0 skip, 1 lo, 2 bias, 3 none)
   __shared__ int sPix[WG_K][4];          // img, z, y, x (img < 0: past the end)
-  const int Cin = A.c_skip + A.c_lo, taps = A.kz * A.kyx * A.kyx;
+  const int Cin = A.c_skip + A.c_lo, taps = A.kz * A.ky * A.kx;
   const int n_ct = (A.cout + WG_C - 1) / WG_C;
   const int r0 = (blockIdx.x / n_ct) * WG_R, c0 = (blockIdx.x % n_ct) * WG_C;
   const int t = threadIdx.x, tr = t / 16, tc = t % 16;
-  const int hz = A.kz / 2, hyx = A.kyx / 2;
   if (t < WG_R) {
     const int r = r0 + t;
     int* q = sRow[t];
     if (r < taps * Cin) {
       const int tap = r / Cin, c = r % Cin;
-      q[0] = tap / (A.kyx * A.kyx) - hz; q[1] = (tap / A.kyx) % A.kyx - hyx; q[2] = tap % A.kyx - hyx;
+      q[0] = tap / (A.ky * A.kx) - A.pz; q[1] = (tap / A.kx) % A.ky - A.py; q[2] = tap % A.kx - A.px;
       q[3] = c < A.c_lo ? c : c - A.c_lo; q[4] = c < A.c_lo ? 1 : 0;
     } else {
       q[0] = q[1] = q[2] = q[3] = 0; q[4] = (r == taps * Cin) ? 2 : 3;
@@ -143,7 +146,7 @@ int wgrad_split(long long npix, int rows, int cout, long long* per_split) {
 }
 
 // ------------------------------------------------------------------------------------------ small elementwise kernels
-// Wf[taps-1-tap][co][ci] = W[tap][ci][co]: flipping every spatial axis of a 3^d (or 1^d) kernel reverses the linear tap index
+// Wf[taps-1-tap][co][ci] = W[tap][ci][co]: flipping every spatial axis of a (kz, ky, kx) box reverses the linear tap index
 __global__ void k_flip_weights(const float* __restrict__ w, int taps, int cin, int cout, float* __restrict__ wf) {
   const long long total = (long long)taps * cin * cout;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
@@ -461,32 +464,51 @@ extern "C" long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin,
   return (long long)ns * rows * cout;
 }
 
-extern "C" int sdb_conv_wgrad_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
-                                 int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
-                                 long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_nd: kernel must be 1^d or 3^d"); return 1; }
+namespace {
+
+int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+               int uz, int uy, int ux, int kz, int ky, int kx, const float* d_dy, int ldy, int cout, float* d_work,
+               long long work_floats, float* d_dw, float* d_db, cudaStream_t st) {
   if (n < 1 || d < 1 || h < 1 || w < 1 || cout < 1 || ldy < cout || cin_skip < 0 || cin_lo < 0 || cin_skip + cin_lo < 1) {
-    sdb::set_error("conv_wgrad_nd: bad arguments"); return 1;
+    sdb::set_error(std::string(who) + ": bad arguments"); return 1;
   }
   if (cin_lo && (d_x_lo == nullptr || uz < 1 || uy < 1 || ux < 1 || d % uz || h % uy || w % ux)) {
-    sdb::set_error("conv_wgrad_nd: low-resolution source needs a pointer and divisible up-sampling factors"); return 1;
+    sdb::set_error(std::string(who) + ": low-resolution source needs a pointer and divisible up-sampling factors"); return 1;
   }
   WgradArgs A;
   A.x = d_x; A.x_lo = d_x_lo; A.dy = d_dy;
   A.n = n; A.d = d; A.h = h; A.w = w; A.c_skip = cin_skip; A.c_lo = cin_lo;
   A.uz = cin_lo ? uz : 1; A.uy = cin_lo ? uy : 1; A.ux = cin_lo ? ux : 1;
-  A.kz = kz; A.kyx = kyx; A.ldy = ldy; A.cout = cout;
-  const int taps = kz * kyx * kyx;
+  A.kz = kz; A.ky = ky; A.kx = kx; A.pz = (kz - 1) / 2; A.py = (ky - 1) / 2; A.px = (kx - 1) / 2;
+  A.ldy = ldy; A.cout = cout;
+  const int taps = kz * ky * kx;
   A.rows = taps * (cin_skip + cin_lo) + 1;
   A.npix = (long long)n * d * h * w;
   const int ns = wgrad_split(A.npix, A.rows, cout, &A.per_split);
-  if ((long long)ns * A.rows * cout > work_floats) { sdb::set_error("conv_wgrad_nd: workspace too small"); return 1; }
+  if ((long long)ns * A.rows * cout > work_floats) { sdb::set_error(std::string(who) + ": workspace too small"); return 1; }
   A.work = d_work;
   dim3 grid(cdiv(A.rows, WG_R) * cdiv(cout, WG_C), ns);
   SDB_LAUNCH(k_conv_wgrad, grid, 256, 0, st, A);
   SDB_LAUNCH(k_wgrad_reduce, grid_1d((long long)A.rows * cout, 16), 256, 0, st, d_work, ns, A.rows, cout, d_dw, d_db);
   return 0;
+}
+
+}  // namespace
+
+extern "C" int sdb_conv_wgrad_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                                 int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
+                                 long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
+  if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_nd: kernel must be 1^d or 3^d"); return 1; }
+  return conv_wgrad("conv_wgrad_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, kyx, kyx, d_dy, ldy, cout, d_work,
+                    work_floats, d_dw, d_db, (cudaStream_t)stream);
+}
+
+extern "C" int sdb_conv_wgrad_any_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                                     int uz, int uy, int ux, int kz, int ky, int kx, const float* d_dy, int ldy, int cout, float* d_work,
+                                     long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
+  if (kz < 1 || kz > 7 || ky < 1 || ky > 7 || kx < 1 || kx > 7) { sdb::set_error("conv_wgrad_any_nd: kernel extents must be in 1..7"); return 1; }
+  return conv_wgrad("conv_wgrad_any_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, ky, kx, d_dy, ldy, cout, d_work,
+                    work_floats, d_dw, d_db, (cudaStream_t)stream);
 }
 
 extern "C" int sdb_conv_flip_weights(const float* d_w, int taps, int cin, int cout, float* d_wf, sdb_stream_t stream) {

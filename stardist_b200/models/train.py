@@ -26,11 +26,12 @@ def check_trainable(config, optimizer=None):
         raise NotImplementedError("unet_batch_norm=True is not supported")
     if optimizer is not None:
         raise NotImplementedError("optimizer=%r: only the default Adam(train_learning_rate) is supported" % (optimizer,))
-    if tuple(config.unet_kernel_size) != (3,) * config.n_dim:
-        raise NotImplementedError("unet_kernel_size=%r: only 3^d kernels are supported" % (tuple(config.unet_kernel_size),))
-    acts = {config.unet_activation, config.unet_last_activation}
-    if not acts <= {'relu', 'linear'}:
-        raise NotImplementedError("activations %s: only 'relu' and 'linear' are supported" % sorted(acts))
+    ks = tuple(int(v) for v in config.unet_kernel_size)
+    if len(ks) != config.n_dim or not all(1 <= v <= 7 for v in ks):
+        raise NotImplementedError("unet_kernel_size=%r: kernel extents 1..7 per axis are supported" % (ks,))
+    from .unet_device import act_id
+    for a in (config.unet_activation, config.unet_last_activation):
+        act_id(a)
     if getattr(config, 'n_classes', None) is not None:
         from .weights import unet_layers
         if config.n_classes + 1 > 32:
@@ -94,9 +95,6 @@ class UNetTrainer:
         self._bufs = {}
         if self.n_classes is not None:
             self.class_w = torch.from_numpy(np.asarray(config.train_class_weights, np.float32)).to(dev)
-        for l in self.layers[1:]:
-            if l['kind'] in ('conv', 'conv_class') and l['cin'] % 32:
-                raise NotImplementedError("layer %s: %d input channels; the input gradient needs a multiple of 32" % (l['name'], l['cin']))
 
     # ---------------------------------------------------------------------------------------------- buffers
     def _buf(self, key, shape, zero=False):
@@ -118,17 +116,22 @@ class UNetTrainer:
         return (1,) + tuple(t.shape[1:3]) if t.dim() == 4 else tuple(t.shape[1:4])
 
     # ---------------------------------------------------------------------------------------------- kernels
-    def _wgrad(self, x, lo, up, k3, dy, ldy, cout, dw, db):
+    def _wgrad(self, x, lo, up, k, dy, ldy, cout, dw, db):
+        """weight and bias gradient of a stride-1 'same' convolution with kernel extents k over the input [upsample(lo), x]"""
+        from .unet_device import conv_wgrad_accepts
         lib = L.load()
         n = x.shape[0]; d, h, w = self._dhw(x)
         c_skip = x.shape[-1]; c_lo = 0 if lo is None else lo.shape[-1]
-        kz = 3 if (k3 and self.nd == 3) else 1
-        kyx = 3 if k3 else 1
+        kz, ky, kx = ((1,) + tuple(k)) if self.nd == 2 else tuple(k)
         uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
-        need = int(lib.sdb_conv_wgrad_workspace(n * d * h * w, kz * kyx * kyx, c_skip + c_lo, cout))
+        need = int(lib.sdb_conv_wgrad_workspace(n * d * h * w, kz * ky * kx, c_skip + c_lo, cout))
         work = self._workspace(need)
-        L.check(lib.sdb_conv_wgrad_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, kyx, L.ptr(dy), ldy, cout,
-                                      L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
+        if conv_wgrad_accepts(self.nd, k):
+            L.check(lib.sdb_conv_wgrad_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, L.ptr(dy), ldy,
+                                          cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
+        else:
+            L.check(lib.sdb_conv_wgrad_any_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, kx, L.ptr(dy),
+                                              ldy, cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
 
     def _loss(self, prob, dist, prob_t, dam, dhead, out, state):
         lib = L.load()
@@ -154,19 +157,35 @@ class UNetTrainer:
         L.check(lib.sdb_stardist_class_loss(L.ptr(s), L.ptr(pc_t), npix, C, L.ptr(self.class_w), float(self.config.train_loss_weights[2]),
                                             L.ptr(work), L.ptr(dclass), L.ptr(out[0:1]), L.ptr(out[4:5]), L.stream_ptr()))
 
-    def _dgrad(self, key, name, g, x_shape, cin, cout):
-        """input gradient of the 3^d convolution `name` (x_shape [..., cin] -> cout): sdb_conv3_nd of g with the flipped kernel"""
+    def _dgrad(self, key, name, g, x_shape, cin, cout, k):
+        """input gradient of the stride-1 convolution `name` (kernel extents k, x_shape [..., cin] -> cout): the correlation of g
+        with the flipped kernel, on sdb_conv3_nd where conv_dgrad3_accepts takes the layer, else on sdb_conv_dgrad_any_nd"""
+        from .unet_device import conv_dgrad3_accepts
         lib = L.load()
         st = L.stream_ptr()
-        taps = 3 ** self.nd
+        taps = int(np.prod(k))
         wf = self._buf(('wflip', key), (taps, cout, cin))
         L.check(lib.sdb_conv_flip_weights(L.ptr(self.pview[name][0]), taps, cin, cout, L.ptr(wf), st))
-        zb = self._buf(('zero_bias', cin), (cin,), zero=True)
         n = x_shape[0]; d, h, w = (1,) + tuple(x_shape[1:3]) if len(x_shape) == 4 else tuple(x_shape[1:4])
         gin = self._buf(('gin', key), tuple(x_shape[:-1]) + (cin,))
-        L.check(lib.sdb_conv3_nd(L.ptr(g), None, n, d, h, w, cout, 0, 1, 1, 1, L.ptr(wf), L.ptr(zb), cin,
-                                 1 if self.nd == 2 else 3, 0, L.ptr(gin), st))
+        if conv_dgrad3_accepts(self.nd, k, cin, cout):
+            zb = self._buf(('zero_bias', cin), (cin,), zero=True)
+            L.check(lib.sdb_conv3_nd(L.ptr(g), None, n, d, h, w, cout, 0, 1, 1, 1, L.ptr(wf), L.ptr(zb), cin,
+                                     1 if self.nd == 2 else 3, 0, L.ptr(gin), st))
+        else:
+            kz, ky, kx = ((1,) + tuple(k)) if self.nd == 2 else tuple(k)
+            L.check(lib.sdb_conv_dgrad_any_nd(L.ptr(g), n, d, h, w, cout, L.ptr(wf), cin, kz, ky, kx, L.ptr(gin), st))
         return gin
+
+    def _act_backward(self, g, act, y, z):
+        """g *= act'(pre-activation) in place: from the output y for ReLU, from the kept pre-activation z for the activations
+        other than ReLU / linear"""
+        lib = L.load()
+        if act == 'relu':
+            L.check(lib.sdb_relu_backward(L.ptr(g), L.ptr(y), g.numel(), L.stream_ptr()))
+        elif act != 'linear':
+            from .unet_device import act_id
+            L.check(lib.sdb_act_backward(L.ptr(g), L.ptr(z), g.numel(), act_id(act), L.stream_ptr()))
 
     def _class_backward(self, dclass, g):
         """the class branch's parameter gradients from dclass = dL/d(softmax logits) per output pixel.  Returns the input
@@ -178,16 +197,19 @@ class UNetTrainer:
         C = self.n_classes + 1
         cf = xc.shape[-1]; npix = xc.numel() // cf
         ones = (1,) * self.nd
-        self._wgrad(xc, None, ones, False, dclass, C, C, *self.gview['prob_class'])
+        self._wgrad(xc, None, ones, ones, dclass, C, C, *self.gview['prob_class'])
         wc = self.pview['prob_class'][0]
         if 'features_class' not in self.pview:
             L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 0, 1, L.ptr(g), st))
             return None
         gc = self._buf('dfeat_class', xc.shape)
-        relu = 1 if self.config.unet_activation == 'relu' else 0
-        L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, relu, 0, L.ptr(gc), st))
-        self._wgrad(base, None, ones, True, gc, cf, cf, *self.gview['features_class'])
-        return self._dgrad('class', 'features_class', gc, base.shape, base.shape[-1], cf)
+        act = self.config.unet_activation
+        L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 1 if act == 'relu' else 0, 0, L.ptr(gc), st))
+        if act != 'relu':
+            self._act_backward(gc, act, xc, self.net.saved_class_z)
+        k = tuple(self.pview['features_class'][0].shape[:self.nd])
+        self._wgrad(base, None, ones, k, gc, cf, cf, *self.gview['features_class'])
+        return self._dgrad('class', 'features_class', gc, base.shape, base.shape[-1], cf, k)
 
     def _backward(self, dhead, dclass=None):
         """gradient of every parameter into self.grad from dhead = (dL/d prob logit, dL/d dist) and, for multi-class models,
@@ -200,8 +222,8 @@ class UNetTrainer:
         cf = feat.shape[-1]; npix = feat.numel() // cf
         ones = (1,) * self.nd
         dh = dhead.view(-1)
-        self._wgrad(feat, None, ones, False, dh, R + 1, 1, *self.gview['prob'])
-        self._wgrad(feat, None, ones, False, dh[1:], R + 1, R, *self.gview['dist'])
+        self._wgrad(feat, None, ones, ones, dh, R + 1, 1, *self.gview['prob'])
+        self._wgrad(feat, None, ones, ones, dh[1:], R + 1, R, *self.gview['dist'])
         g = self._buf('dfeat', feat.shape)
         L.check(lib.sdb_heads_backward(L.ptr(feat), L.ptr(dhead), npix, cf, L.ptr(self.pview['prob'][0]), L.ptr(self.pview['dist'][0]),
                                        R, 0, L.ptr(g), st))
@@ -212,15 +234,14 @@ class UNetTrainer:
             l = self.layers[i]
             a = net.saved[i]
             if l['kind'] == 'conv':
-                if l['act'] == 'relu':
-                    L.check(lib.sdb_relu_backward(L.ptr(g), L.ptr(a['y']), g.numel(), st))
+                self._act_backward(g, l['act'], a['y'], a['z'])
                 x, lo, up = a['x'], a['lo'], a['up']
                 cout = l['cout']
-                self._wgrad(x, lo, up, True, g, cout, cout, *self.gview[l['name']])
+                self._wgrad(x, lo, up, l['k'], g, cout, cout, *self.gview[l['name']])
                 if i == first:
                     break                                    # the network input needs no gradient
                 n = x.shape[0]; d, h, w = self._dhw(x)
-                gin = self._dgrad(i, l['name'], g, x.shape, l['cin'], cout)
+                gin = self._dgrad(i, l['name'], g, x.shape, l['cin'], cout, l['k'])
                 if gin_class is not None and l['name'] == 'features':
                     L.check(lib.sdb_add_act(L.ptr(gin), L.ptr(gin_class), gin.numel(), 0, L.ptr(gin), st))
                 if lo is not None:

@@ -63,6 +63,27 @@ def add_act_accepts(act):
     return act in ('relu', 'linear')
 
 
+# Training (csrc/unet_train.cu): the layers these predicates accept take the backward kernels of the default family, every
+# other layer the unet_any.cu / any-extent entry points.
+def conv_wgrad_accepts(nd, k):
+    """sdb_conv_wgrad_nd: 1^d and 3^d kernels, and (1, 3, 3) in 3-D; sdb_conv_wgrad_any_nd takes every other extent"""
+    k = tuple(k)
+    return k in ((1,) * nd, (3,) * nd) or (nd == 3 and k == (1, 3, 3))
+
+
+def conv_dgrad3_accepts(nd, k, cin, cout):
+    """input gradient as sdb_conv3_nd of dY (cout channels) with the flipped kernel (cin outputs): 3^d kernels whose
+    transposed shape that kernel takes (in particular every cin % 32 == 0 layer with cout a multiple of 8); every other layer
+    runs sdb_conv_dgrad_any_nd"""
+    return conv3_accepts(nd, k, (1,) * nd, cout, 0, cin, 'linear')
+
+
+def keeps_preactivation(act):
+    """training keeps the pre-activation z of layers whose activation derivative needs it (every activation but ReLU and
+    linear, whose backward reads the output)"""
+    return act not in ('relu', 'linear')
+
+
 class UNetDeviceND:
     """exact-fp32 CUDA-core executor for 2-D (NHWC) and 3-D (NDHWC) U-Nets: csrc/unet_simt.cu for the layers its kernels
     accept (see the *_accepts predicates), csrc/unet_any.cu for every other kernel extent, channel count, feature width and
@@ -89,8 +110,10 @@ class UNetDeviceND:
     def _dhw(x):
         return (1,) + tuple(x.shape[1:3]) if x.dim() == 4 else tuple(x.shape[1:4])
 
-    def _conv(self, x, x_lo, name, act, up, stride=None):
-        """act(conv(x) + bias) with 'same' padding; the input channels are [upsample(x_lo), x] when x_lo is given"""
+    def _conv(self, x, x_lo, name, act, up, stride=None, keep_z=False):
+        """act(conv(x) + bias) with 'same' padding; the input channels are [upsample(x_lo), x] when x_lo is given.
+        keep_z=True (activations other than ReLU / linear) returns (z, act(z)): the same kernel runs linear and sdb_act_any
+        applies the activation, which gives the fused result bit for bit."""
         lib = L.load()
         k, b = self.w[name]
         n = x.shape[0]; d, h, w = self._dhw(x); c_skip = x.shape[-1]
@@ -101,6 +124,7 @@ class UNetDeviceND:
         stride = (1,) * self.nd if stride is None else tuple(stride)
         uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
         if conv3_accepts(self.nd, ks, stride, c_skip, c_lo, cout, act):
+            assert not keep_z
             out = torch.empty(tuple(x.shape[:-1]) + (cout,), dtype=torch.float32, device=x.device)
             L.check(lib.sdb_conv3_nd(L.ptr(x), L.ptr(x_lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), L.ptr(k), L.ptr(b), cout,
                                     1 if self.nd == 2 else 3, 1 if act == 'relu' else 0, L.ptr(out), L.stream_ptr()))
@@ -109,26 +133,34 @@ class UNetDeviceND:
         osp = tuple(-(-s // t) for s, t in zip(x.shape[1:-1], stride))
         out = torch.empty((n,) + osp + (cout,), dtype=torch.float32, device=x.device)
         L.check(lib.sdb_conv_any_nd(L.ptr(x), L.ptr(x_lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), L.ptr(k), L.ptr(b), cout,
-                                   kz, ky, kx, sz, sy, sx, act_id(act), L.ptr(out), L.stream_ptr()))
+                                   kz, ky, kx, sz, sy, sx, 0 if keep_z else act_id(act), L.ptr(out), L.stream_ptr()))
+        if keep_z:
+            y = torch.empty_like(out)
+            L.check(lib.sdb_act_any(L.ptr(out), out.numel(), act_id(act), L.ptr(y), L.stream_ptr()))
+            return out, y
         return out
 
     def _class_branch(self, base, keep=False):
         """prob_class [N,...,n_classes+1] from the backbone output `base` (fp32, channels last), or None.  keep=True stores
-        self.saved_class = (base, the prob_class layer's input, prob_class) for the backward pass."""
+        self.saved_class = (base, the prob_class layer's input, prob_class) for the backward pass, and in
+        self.saved_class_z the pre-activation of features_class when its activation is neither ReLU nor linear."""
         if self.config.n_classes is None:
             return None
         lib = L.load()
-        x = base
+        x, z = base, None
         if 'features_class' in self.w:
             act = self.config.unet_activation if getattr(self.config, 'backbone', 'unet') == 'unet' else self.config.resnet_activation
-            x = self._conv(base, None, 'features_class', act, (1,) * self.nd)
+            if keep and keeps_preactivation(act):
+                z, x = self._conv(base, None, 'features_class', act, (1,) * self.nd, keep_z=True)
+            else:
+                x = self._conv(base, None, 'features_class', act, (1,) * self.nd)
         wc, bc = self.w['prob_class']
         C = int(wc.shape[-1]); cf = int(x.shape[-1])
         npix = int(np.prod(x.shape[:-1]))
         out = torch.empty(tuple(x.shape[:-1]) + (C,), dtype=torch.float32, device=x.device)
         L.check(lib.sdb_class_head(L.ptr(x), npix, cf, L.ptr(wc.reshape(cf, C).contiguous()), L.ptr(bc), C, L.ptr(out), L.stream_ptr()))
         if keep:
-            self.saved_class = (base, x, out)
+            self.saved_class, self.saved_class_z = (base, x, out), z
         return out
 
     def _pool(self, x, pool):
@@ -156,8 +188,9 @@ class UNetDeviceND:
     def forward(self, x, keep=False):
         """x: float32 [N,(D,)H,W,Cin] on the device -> (prob [N,...], dist [N,...,R]).
         keep=True stores in self.saved, per entry of self.layers, what the backward pass reads: for a convolution its
-        inputs (x, x_lo, up) and its output y, for a pooling its input x; self.saved_feat is the heads' input and, for
-        multi-class models, self.saved_class the class branch's (see _class_branch)."""
+        inputs (x, x_lo, up), its output y and, for activations other than ReLU / linear, its pre-activation z (the layer then
+        runs linear and its activation as a separate pass, with the same y), for a pooling its input x; self.saved_feat is
+        the heads' input and, for multi-class models, self.saved_class the class branch's (see _class_branch)."""
         assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
         skips = {}
         lo, up = None, (1,) * self.nd
@@ -167,9 +200,12 @@ class UNetDeviceND:
             kind = l['kind']
             if kind == 'conv':
                 if l['name'] == 'features': base = x
-                y = self._conv(x, lo, l['name'], l['act'], up)
+                if keep and keeps_preactivation(l['act']):
+                    z, y = self._conv(x, lo, l['name'], l['act'], up, keep_z=True)
+                else:
+                    z, y = None, self._conv(x, lo, l['name'], l['act'], up)
                 if keep:
-                    saved[i] = dict(x=x, lo=lo, up=up, y=y)
+                    saved[i] = dict(x=x, lo=lo, up=up, y=y, z=z)
                 x = y
                 lo, up = None, (1,) * self.nd
             elif kind == 'pool':
