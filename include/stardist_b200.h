@@ -234,6 +234,20 @@ int sdb_train_gather(const long long* d_items, const int* d_pos, int ndim, int b
 int sdb_class_map(const int* d_y_slots, int ndim, int batch, const int* patch_size, const int* d_zoom_index,
                   const int* out_shape, const int* d_class_table, int n_classes, const unsigned char* d_neg, float* d_out,
                   sdb_stream_t stream);
+/* The training notebooks' augmenter (augment.cu, DESIGN.md 4.2).  sdb_mt_normal: np.random.normal(0, 1, n) of numpy's legacy
+ * RandomState from its state (h_key [624], pos, has_gauss, gauss as get_state() gives them) -> d_out float64 [n] and the state
+ * numpy holds afterwards (h_key_out may be h_key); synchronises the stream.  Values may differ from numpy's by the ulps of
+ * the device's double log; the state is numpy's.  sdb_augment_batch: per item b the output patch of d_params int64 [batch][12]
+ * = (source axis of output axis 0..2, flip of output axis 0..2, float32 bits of scale and shift, float64 bits of sigma, noise
+ * on, 0, 0), axes counted with a leading unit axis in 2-D; from the gathered d_x [batch][patch][n_channels], raw labels d_y_raw
+ * and slots d_y_slots (sdb_train_gather with clamp 0) it writes d_x_out = x * s + t (float32), plus float32(double(.) +
+ * sigma * d_noise[b][patch][n_channels]) with noise on, d_y_clamped = max(label, 0), d_y_slots_out, and at the grid positions
+ * d_neg (label < 0) and, if not NULL, d_y_slots_grid -- what sdb_train_gather writes for the augmented patch. */
+int sdb_mt_normal(const unsigned* h_key, int pos, int has_gauss, double gauss, long long n, double* d_out, unsigned* h_key_out,
+                  int* h_pos_out, int* h_has_gauss_out, double* h_gauss_out, sdb_stream_t stream);
+int sdb_augment_batch(const long long* d_params, int ndim, int batch, const int* patch_size, int n_channels, const int* grid,
+                      const float* d_x, const int* d_y_raw, const int* d_y_slots, const double* d_noise, float* d_x_out,
+                      int* d_y_clamped, int* d_y_slots_out, int* d_y_slots_grid, unsigned char* d_neg, sdb_stream_t stream);
 /* host-pointer versions on any int32 label map (negative labels are never an object; relabelling, the constant-image rule and
  * the mapping back to the original labels happen inside): void, on failure the result is zeroed and sdb_last_error() holds
  * the message (cleared on success) */

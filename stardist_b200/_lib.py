@@ -156,6 +156,10 @@ def _declare(lib):
     lib.sdb_train_gather.restype = c_int
     lib.sdb_class_map.argtypes = [P, c_int, c_int, P, P, P, P, c_int, P, P, P]
     lib.sdb_class_map.restype = c_int
+    lib.sdb_mt_normal.argtypes = [P, c_int, c_int, c_double, c_longlong, P, P, POINTER(c_int), POINTER(c_int), POINTER(c_double), P]
+    lib.sdb_mt_normal.restype = c_int
+    lib.sdb_augment_batch.argtypes = [P, c_int, c_int, P, c_int, P, P, P, P, P, P, P, P, P, P, P]
+    lib.sdb_augment_batch.restype = c_int
     lib.sdb_fill_label_holes.argtypes = [P, c_int, P, c_int, c_int, P, P]
     lib.sdb_fill_label_holes.restype = c_int
     lib._LIB_edt_prob.argtypes = [P, c_int, P, P, P]

@@ -33,8 +33,13 @@ NotImplementedError, and an X / Y without len() / __getitem__ ValueError; class 
 reads of one lazy image with different shapes (the reference would crop one at positions valid for the other) raise
 ValueError.  A label of a patch that has no class in the dict raises the reference's ValueError when that batch is made.
 X is returned as float32 even when an augmenter returns another float type.
+
+An Augmenter (models/augment.py) runs on the device: after the gather (labels not clamped), sdb_augment_batch transposes, flips
+and rescales every item's patch and adds its noise, which sdb_mt_normal draws from np.random's stream; the targets follow as
+without augmentation.  Any other callable augmenter gets numpy patches on the host, and its results are relabelled and gathered
+again.
 """
-import random, threading, warnings
+import random, threading, warnings, weakref
 import numpy as np
 
 from .. import _lib as L
@@ -144,6 +149,12 @@ def _class_code(cls, n_classes):
     raise ValueError(f"Wrong class id '{cls}' (for n_classes={n_classes})")
 
 
+def _weak_method(method):
+    """a callable for a bound method that does not keep its object alive"""
+    ref = weakref.WeakMethod(method)
+    return lambda *args: ref()(*args)
+
+
 def _is_resident(X):
     return isinstance(X, (np.ndarray, tuple, list))
 
@@ -249,9 +260,14 @@ class _StarDistDataDevice(RollingSequence):
                 raise AssertionError("all images must have the same number of channels")
         if not (0 <= foreground_prob <= 1):
             raise AssertionError("foreground_prob must lie in [0, 1]")
+        from .augment import Augmenter
+        self._aug_device = self._aug_axis = None
         if augmenter is None:
             self._augment = False
             augmenter = lambda *args: args
+        elif isinstance(augmenter, Augmenter):
+            self._augment = False
+            self._aug_device, self._aug_axis = augmenter, augmenter.checked_axis(patch_size)
         else:
             callable(augmenter) or _raise(ValueError("augmenter must be None or callable"))
             self._augment = True
@@ -292,7 +308,10 @@ class _StarDistDataDevice(RollingSequence):
         self._lazy, self._stage, self._stage_done = None, None, None
         if not resident:
             # lazy dataset: nothing is read or uploaded until a batch needs it
-            self._lazy = LazyReads(X, Y, self.patch_size, sample_ind_cache, self._check_item, self._check_valid_mask, self._fg_index)
+            # weak references back to the generator: without a reference cycle, a dropped generator frees its cached
+            # foreground masks at once, not whenever the cyclic garbage collector next runs
+            self._lazy = LazyReads(X, Y, self.patch_size, sample_ind_cache, *(_weak_method(m) for m in (
+                self._check_item, self._check_valid_mask, self._fg_index)))
             return
         # resident dataset: X float32 [..., C], Y int32, the sequential relabelling of Y and its label count
         for k, (x, y) in enumerate(zip(X, Y)):
@@ -487,8 +506,11 @@ class _StarDistDataDevice(RollingSequence):
                 lab = labels.cpu().numpy()
                 cls_table = np.concatenate([np.zeros(1, np.int32)] + [self._class_table(self.classes[k], lab)[1:] for k, _, _ in plan])
         d_cls = torch.from_numpy(cls_table).to(dev) if classes_on else None
-        L.check(lib.sdb_train_gather(L.ptr(items), L.ptr(pos), nd, B, L.iarr(p), C, L.iarr(g), L.ptr(d_cls), L.ptr(x), L.ptr(yc), L.ptr(ys),
-                                     L.ptr(ye), L.ptr(neg), L.ptr(status), 1, L.stream_ptr()))
+        if self._aug_device is not None:
+            self._augment_on_device(items, pos, d_cls, status, x, yc, ys, ye, neg)
+        else:
+            L.check(lib.sdb_train_gather(L.ptr(items), L.ptr(pos), nd, B, L.iarr(p), C, L.iarr(g), L.ptr(d_cls), L.ptr(x), L.ptr(yc), L.ptr(ys),
+                                         L.ptr(ye), L.ptr(neg), L.ptr(status), 1, L.stream_ptr()))
         del res                # a lazy batch's images are not read past the gather (their memory is reused in stream order)
         R = self.n_rays
         dam = torch.empty((B,) + pg + (R + 1,), dtype=torch.float32, device=dev)
@@ -510,6 +532,28 @@ class _StarDistDataDevice(RollingSequence):
             L.check(lib.sdb_class_map(L.ptr(ys), nd, B, L.iarr(p), L.ptr(self._zoom), L.iarr(self._zoom_shape), L.ptr(d_cls), self.n_classes,
                                       L.ptr(neg), L.ptr(prob_class), L.stream_ptr()))
         return x, prob, dam, prob_class, status
+
+    def _augment_on_device(self, items, pos, d_cls, status, x, yc, ys, ye, neg):
+        """the gather and the Augmenter: x, yc, ys, ye, neg as sdb_train_gather writes them, for the augmented patches"""
+        import torch
+        lib = L.require_cuda()
+        B, nd, p, g = x.shape[0], self.ndim, self.patch_size, self.grid
+        C = x.shape[-1]
+        xr, yr, sr = torch.empty_like(x), torch.empty_like(yc), torch.empty_like(ys)
+        L.check(lib.sdb_train_gather(L.ptr(items), L.ptr(pos), nd, B, L.iarr(p), C, L.iarr(g), L.ptr(d_cls), L.ptr(xr), L.ptr(yr), L.ptr(sr),
+                                     None, L.ptr(neg), L.ptr(status), 0, L.stream_ptr()))
+        from .augment import normal_device
+        aug = self._aug_device
+        noise = None if aug.noise is None else torch.empty((B, xr[0].numel()), dtype=torch.float64, device="cuda")
+        rows = []
+        for b in range(B):             # the notebooks' draws, item after item; the noise of an item before the next item draws
+            row, sig = aug.draw(self._aug_axis, nd)
+            if sig is not None:
+                normal_device(noise.shape[1], noise[b])
+            rows.append(row)
+        prm = torch.from_numpy(np.asarray(rows, np.int64)).to("cuda")
+        L.check(lib.sdb_augment_batch(L.ptr(prm), nd, B, L.iarr(p), C, L.iarr(g), L.ptr(xr), L.ptr(yr), L.ptr(sr), L.ptr(noise), L.ptr(x),
+                                      L.ptr(yc), L.ptr(ys), L.ptr(ye), L.ptr(neg), L.stream_ptr()))
 
     def _finish(self, status):
         """the host side of the batch's single read-back: the constant-patch warning per item, the missing-class error"""
