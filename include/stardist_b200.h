@@ -155,6 +155,26 @@ int sdb_relabel_sequential(int* d_labels, long long n, int max_label, int offset
 int sdb_label_overlap(const int* d_a, const int* d_b, long long n, int* d_pairs, long long* d_counts,
                       long long capacity, long long* h_n_pairs, sdb_stream_t stream);
 
+/* group_matching_labels (stardist/matching.py:409-472) on an int32 stack d_stack[n_frames][frame_size]; the three calls
+ * share the table machinery and capacity protocol of sdb_label_overlap (d_keys / d_counts [capacity], *h_n_keys after one
+ * stream synchronisation, > capacity = nothing written and an upper bound returned; negative labels are an error).
+ * sdb_stack_labels: every distinct (frame, label) of the stack, background 0 included, as the sorted keys
+ *   (frame << 32) | label with their pixel counts.
+ * sdb_stack_overlap: the overlap tables of the frame pairs (p, p + 1), p in [first_pair, first_pair + n_pairs), on ids
+ *   compacted per frame as relabel_sequential numbers them (0 stays 0, the non-zero labels of frame f become 1..n_f in
+ *   ascending order): d_ids holds the sorted non-zero labels of every frame, those of frame f at
+ *   [d_offsets[f], d_offsets[f + 1]).  Sorted keys ((p - first_pair) << 2 key_bits) | (a' << key_bits) | b' with their
+ *   pixel counts; key_bits in [1, 31] must hold every compacted id, and n_pairs - 1 must fit in 63 - 2 key_bits bits.
+ * sdb_stack_group_remap: d_out[0] = d_stack[0]; d_out[f] = d_lut[d_offsets[f] + a' - 1] where d_stack[f] has a
+ *   compacted id a' > 0, else 0 (d_lut is laid out like d_ids).  Asynchronous. */
+int sdb_stack_labels(const int* d_stack, long long n_frames, long long frame_size, long long* d_keys, long long* d_counts,
+                     long long capacity, long long* h_n_keys, sdb_stream_t stream);
+int sdb_stack_overlap(const int* d_stack, long long frame_size, long long first_pair, long long n_pairs, const int* d_ids,
+                      const long long* d_offsets, int key_bits, long long* d_keys, long long* d_counts, long long capacity,
+                      long long* h_n_keys, sdb_stream_t stream);
+int sdb_stack_group_remap(const int* d_stack, long long n_frames, long long frame_size, const int* d_ids,
+                          const long long* d_offsets, const int* d_lut, int* d_out, sdb_stream_t stream);
+
 /* star distances (stardist2d.cpp:55-125 c_star_dist, stardist3d.cpp:245-345 c_star_dist3d), bit-identical to the reference.
  * d_labels: label map [H, W] / [D, H, W], uint16 (label_bytes 2) or int32 (label_bytes 4); labels are compared by their low
  * 16 bits (the reference's astype(np.uint16)).  h_dirs: HOST float32 table [2][n_rays] = [dy | dx] (dy = cosf(phi_k),

@@ -130,6 +130,12 @@ def _declare(lib):
     lib.sdb_relabel_sequential.restype = c_int
     lib.sdb_label_overlap.argtypes = [P, P, c_longlong, P, P, c_longlong, POINTER(c_longlong), P]
     lib.sdb_label_overlap.restype = c_int
+    lib.sdb_stack_labels.argtypes = [P, c_longlong, c_longlong, P, P, c_longlong, POINTER(c_longlong), P]
+    lib.sdb_stack_labels.restype = c_int
+    lib.sdb_stack_overlap.argtypes = [P, c_longlong, c_longlong, c_longlong, P, P, c_int, P, P, c_longlong, POINTER(c_longlong), P]
+    lib.sdb_stack_overlap.restype = c_int
+    lib.sdb_stack_group_remap.argtypes = [P, c_longlong, c_longlong, P, P, P, P, P]
+    lib.sdb_stack_group_remap.restype = c_int
     lib.sdb_star_dist_2d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_longlong, P, P]
     lib.sdb_star_dist_2d.restype = c_int
     lib.sdb_star_dist_3d.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, P, P, c_longlong, P, P]

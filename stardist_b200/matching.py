@@ -1,6 +1,7 @@
 """relabel_sequential (stardist/matching.py:319-406; itself taken from scikit-image) -- host-side
 integer bookkeeping used by StarDist3D._instances_from_prediction (model3d.py:645) and
 predict_instances_big (base.py:959)."""
+import os
 import numpy as np
 
 from .utils import _raise
@@ -141,18 +142,39 @@ def _ratio(num, den):
     return out
 
 
+def intersection_over_union(overlap):
+    """overlap / (n_pixels_true + n_pixels_pred - overlap) as float32, 0 where the denominator is 0; an all-zero overlap
+    is returned as it is (stardist/matching.py:65-72)"""
+    _check_label_array(overlap, 'overlap')
+    if np.sum(overlap) == 0:
+        return overlap
+    n_pixels_pred = np.sum(overlap, axis=0, keepdims=True)
+    n_pixels_true = np.sum(overlap, axis=1, keepdims=True)
+    return _ratio(overlap, n_pixels_pred + n_pixels_true - overlap)
+
+
+def intersection_over_true(overlap):
+    """overlap / n_pixels_true (row sums) as float32 (stardist/matching.py:77-82)"""
+    _check_label_array(overlap, 'overlap')
+    if np.sum(overlap) == 0:
+        return overlap
+    return _ratio(overlap, np.sum(overlap, axis=1, keepdims=True))
+
+
+def intersection_over_pred(overlap):
+    """overlap / n_pixels_pred (column sums) as float32 (stardist/matching.py:87-92)"""
+    _check_label_array(overlap, 'overlap')
+    if np.sum(overlap) == 0:
+        return overlap
+    return _ratio(overlap, np.sum(overlap, axis=0, keepdims=True))
+
+
+_CRITERION_FUNCTIONS = dict(iou=intersection_over_union, iot=intersection_over_true, iop=intersection_over_pred)
+
+
 def _criterion_scores(overlap, criterion):
-    if overlap.sum() == 0:
-        return overlap.astype(np.float32)
-    n_pred = overlap.sum(axis=0, keepdims=True)
-    n_true = overlap.sum(axis=1, keepdims=True)
-    if criterion == 'iou':
-        return _ratio(overlap, n_pred + n_true - overlap)
-    if criterion == 'iot':
-        return _ratio(overlap, n_true)
-    if criterion == 'iop':
-        return _ratio(overlap, n_pred)
-    raise ValueError("Matching criterion '%s' not supported." % criterion)
+    criterion in _CRITERION_FUNCTIONS or _raise(ValueError("Matching criterion '%s' not supported." % criterion))
+    return _CRITERION_FUNCTIONS[criterion](overlap)
 
 
 def matching_from_overlap(overlap, thresh=0.5, criterion='iou', report_matches=False, map_rev_true=None, map_rev_pred=None):
@@ -269,3 +291,210 @@ def matching_dataset_lazy(y_gen, thresh=0.5, criterion='iou', by_image=False, sh
     stats_all = tuple(matching(y_t, y_p, thresh=threshs, criterion=criterion, report_matches=False) for y_t, y_p in y_gen)
     acc = accumulate_matching(stats_all, threshs, criterion=criterion, by_image=by_image)
     return acc[0] if single else acc
+
+
+# ---------------------------------------------------------------------------------------------------------
+# group_matching_labels (stardist/matching.py:409-472): objects of consecutive frames are linked greedily, frame i + 1 against
+# the grouped frame i.  Grouping only renames the objects of frame i (one-to-one), so the overlap of the original frames i,
+# i + 1 on their compacted ids is the overlap `matching` builds, up to the order of its rows: `matching` relabels the grouped
+# frame sequentially, i.e. rows in ascending order of the grouped ids, and linear_sum_assignment breaks ties by that order.
+# _group_chain therefore re-orders each pair's rows by the grouped ids before the assignment.  The overlap tables come from
+# the device (sdb_stack_overlap) or from numpy; _group_chain serves both.
+_INT32_MAX = int(np.iinfo(np.int32).max)
+
+
+def _compact_labels(y):
+    """(ids, compacted): the sorted non-zero labels of y, and y with each label replaced by 1 + its index in ids (0 stays 0),
+    as int32 -- the numbering of relabel_sequential, without its dense forward map of max(y) + 1 entries"""
+    u, inv = np.unique(y, return_inverse=True)
+    inv = inv.reshape(y.shape).astype(np.int32)
+    if u.size and u[0] == 0:
+        return u[1:], inv
+    return u, inv + 1
+
+
+def _group_chain(ids, overlap, thresh, criterion):
+    """Grouped ids of every object of every frame.  ids[f]: the sorted non-zero labels of frame f; overlap(p): the dense
+    int64 overlap of frames p and p + 1 on their compacted ids, (1 + len(ids[p])) x (1 + len(ids[p + 1])).  Returns luts:
+    luts[f][k] is the grouped id of the label ids[f][k]; frame 0 keeps its labels."""
+    luts = [np.asarray(ids[0], np.int64)]
+    next_id = int(luts[0].max()) + 1 if luts[0].size else 1                       # ys_grouped[0].max() + 1
+    for p in range(len(ids) - 1):
+        g = luts[p]
+        order = np.argsort(g)                                                        # grouped ids are distinct
+        rows = np.concatenate(([0], 1 + order))
+        res = matching_from_overlap(overlap(p)[rows], thresh, criterion, report_matches=True,
+                                    map_rev_true=np.concatenate(([0], g[order])))
+        lut = np.full(len(ids[p + 1]), -1, np.int64)
+        for k in res.matched_tps:
+            gid, j = res.matched_pairs[k]
+            lut[j - 1] = gid
+        new = np.flatnonzero(lut < 0)                                               # ascending label order, as regionprops
+        if new.size and next_id + new.size - 1 > _INT32_MAX:
+            raise ValueError("group_matching_labels: more than 2^31 - 1 label ids are needed (the result is int32)")
+        lut[new] = next_id + np.arange(new.size)
+        next_id += int(new.size)
+        luts.append(lut)
+    return luts
+
+
+def _check_group_input(ys, criterion):
+    """the checks of stardist/matching.py:441-450, then labels below 2^31 and a supported criterion"""
+    len(ys) > 1 or _raise(ValueError("'ys' must have 2 or more entries"))
+    if isinstance(ys, np.ndarray):
+        _check_label_array(ys, 'ys')
+        ys.ndim > 1 or _raise(ValueError("'ys' must be at least 2-dimensional"))
+    else:
+        all(_check_label_array(y, 'ys') for y in ys) or _raise(ValueError("'ys' must be a list of label images"))
+        all(y.shape == ys[0].shape for y in ys) or _raise(ValueError("all label images must have the same shape"))
+    for y in ((ys,) if isinstance(ys, np.ndarray) else ys):
+        if np.iinfo(y.dtype).max > _INT32_MAX and y.size and int(y.max()) > _INT32_MAX:
+            raise ValueError("group_matching_labels: labels must be below 2^31 (the result is int32)")
+    criterion in MATCHING_CRITERIA or _raise(ValueError("Matching criterion '%s' not supported." % criterion))
+
+
+def _device_ready():
+    import torch
+    from . import _lib as L
+    return torch.cuda.is_available() and os.path.exists(L.LIB_PATH)
+
+
+def group_matching_labels(ys, thresh=1e-10, criterion='iou'):
+    """Group matching objects of consecutive label images (e.g. the frames of a time-lapse) under one id
+    (stardist/matching.py:409-472).  Frame i + 1 is matched against the grouped frame i with `matching` (`thresh`,
+    `criterion`); its matched objects take the id of their partner, the others new ids in ascending order of their label,
+    counting up from ys[0].max() + 1.
+
+    ys: an integer array [T, ...] or a list / tuple of equally shaped integer label images, T >= 2, labels in [0, 2^31);
+    returns an np.int32 array [T, ...] whose frame 0 is ys[0].  A contiguous CUDA int32 tensor [T, ...] is also accepted
+    and gives a CUDA int32 tensor; only the per-frame id lists and per-pair overlap tables then leave the device.
+    With the CUDA library the overlaps and the relabelling run on the device, otherwise in numpy; the result is the same."""
+    import torch
+    if isinstance(ys, torch.Tensor):
+        len(ys) > 1 or _raise(ValueError("'ys' must have 2 or more entries"))
+        ys.ndim > 1 or _raise(ValueError("'ys' must be at least 2-dimensional"))
+        if not (ys.is_cuda and ys.dtype == torch.int32 and ys.is_contiguous()):
+            raise ValueError("group_matching_labels expects a contiguous CUDA int32 tensor (or numpy label arrays)")
+        criterion in MATCHING_CRITERIA or _raise(ValueError("Matching criterion '%s' not supported." % criterion))
+        return _group_device(ys, thresh, criterion)
+    _check_group_input(ys, criterion)
+    if _device_ready():
+        stack = torch.from_numpy(np.ascontiguousarray(np.stack([np.asarray(y, np.int32) for y in ys]))).cuda()
+        return _group_device(stack, thresh, criterion).cpu().numpy()
+    return _group_host(ys, thresh, criterion)
+
+
+def _group_host(ys, thresh, criterion):
+    """group_matching_labels on the host: the overlaps from numpy (_overlap_matrix on compacted frames)"""
+    ids, comp = zip(*(_compact_labels(np.asarray(y, np.int32)) for y in ys))
+    luts = _group_chain(ids, lambda p: _overlap_matrix(comp[p], comp[p + 1]), thresh, criterion)
+    out = np.empty((len(ys),) + comp[0].shape, np.int32)
+    out[0] = ys[0]
+    for f in range(1, len(ys)):
+        out[f] = np.concatenate(([0], luts[f]))[comp[f]]
+    return out
+
+
+def _table_device(call, capacity):
+    """(keys, counts) host int64 arrays of one sdb_stack_* table call under the capacity protocol of label_overlap_device,
+    or None when the table needs more than 2^28 entries"""
+    import ctypes, torch
+    from . import _lib as L
+    cap = max(1, min(int(capacity), 1 << 28))
+    for attempt in range(2):
+        keys = torch.empty(cap, dtype=torch.int64, device='cuda')
+        counts = torch.empty(cap, dtype=torch.int64, device='cuda')
+        m = ctypes.c_longlong(0)
+        rc = call(L.ptr(keys), L.ptr(counts), cap, ctypes.byref(m))
+        if rc != 0:
+            if 'negative' in L.load().sdb_last_error().decode('utf-8', 'replace'):
+                raise ValueError("ys must be an array of non-negative integers.")
+            L.check(rc)
+        if m.value <= cap:
+            return keys[:m.value].cpu().numpy(), counts[:m.value].cpu().numpy()
+        if m.value > (1 << 28):
+            return None
+        cap = int(m.value)
+    raise L.StarDistB200Error("stack table: %d keys do not fit the reported bound %d" % (m.value, cap))
+
+
+def stack_labels_device(stack, capacity=1 << 16):
+    """The sorted non-zero labels of every frame of a contiguous CUDA int32 stack [T, ...] (sdb_stack_labels).  Returns
+    host arrays (ids int32, offsets int64 [T + 1]): the labels of frame f are ids[offsets[f]:offsets[f + 1]].  Negative
+    labels raise ValueError."""
+    from . import _lib as L
+    lib = L.require_cuda()
+    T = int(stack.shape[0]); S = stack.numel() // max(T, 1)
+    tab = _table_device(lambda k, c, cap, m: lib.sdb_stack_labels(L.ptr(stack), T, S, k, c, cap, m, L.stream_ptr()), capacity)
+    if tab is None:
+        raise L.StarDistB200Error("stack_labels: more than 2^28 distinct (frame, label) pairs")
+    keys = tab[0]
+    frame, lab = keys >> 32, (keys & 0xffffffff).astype(np.int32)
+    frame, lab = frame[lab != 0], lab[lab != 0]
+    return lab, np.searchsorted(frame, np.arange(T + 1)).astype(np.int64)
+
+
+def stack_overlap_device(stack, ids, offsets, capacity=None, pairs_per_chunk=None):
+    """Overlap tables of every consecutive frame pair of a contiguous CUDA int32 stack [T, ...] on ids compacted per frame
+    (sdb_stack_overlap), in one pass over the stack per chunk of pairs.  `ids`, `offsets`: as stack_labels_device returns
+    them.  Returns a list of T - 1 tuples (a, b, counts) of host int64 arrays, sorted by (a, b), with 0 for the background and
+    k + 1 for the label ids[offsets[f] + k].  The key holds the pair index in the bits the compacted ids leave free; pairs
+    are processed in chunks that fit there, or that `pairs_per_chunk` bounds.  `capacity`: first guess of the number of
+    keys per chunk (default: from the object counts); a short guess costs one repeated call."""
+    import torch
+    from . import _lib as L
+    lib = L.require_cuda()
+    T = int(stack.shape[0]); S = stack.numel() // max(T, 1)
+    n_obj = np.diff(offsets)
+    w = max(1, int(n_obj.max()).bit_length() if n_obj.size else 1)
+    chunk = min(max(T - 1, 1), 1 << min(63 - 2 * w, 40))
+    if pairs_per_chunk is not None:
+        chunk = max(1, min(chunk, int(pairs_per_chunk)))
+    ids_d = torch.from_numpy(np.ascontiguousarray(ids, np.int32)).cuda()
+    off_d = torch.from_numpy(np.ascontiguousarray(offsets, np.int64)).cuda()
+    mask = (1 << w) - 1
+    tables, p = [], 0
+    while p < T - 1:
+        k = min(chunk, T - 1 - p)
+        cap = capacity if capacity is not None else 2 * int(n_obj[p:p + k + 1].sum() + n_obj[p + 1:p + k + 1].sum() + 2 * k)
+        tab = _table_device(lambda kd, cd, c, m: lib.sdb_stack_overlap(L.ptr(stack), S, p, k, L.ptr(ids_d), L.ptr(off_d), w, kd, cd,
+                                                                       c, m, L.stream_ptr()), cap)
+        if tab is None:
+            if k == 1:
+                raise L.StarDistB200Error("stack_overlap: more than 2^28 distinct pairs in one frame pair")
+            chunk = (k + 1) // 2
+            continue
+        keys, counts = tab
+        g = keys >> (2 * w)
+        cuts = np.searchsorted(g, np.arange(k + 1))
+        for q in range(k):
+            kk = keys[cuts[q]:cuts[q + 1]]
+            tables.append(((kk >> w) & mask, kk & mask, counts[cuts[q]:cuts[q + 1]]))
+        p += k
+    return tables
+
+
+def _group_device(stack, thresh, criterion):
+    """group_matching_labels of a contiguous CUDA int32 stack: per-frame ids and overlap tables on the device, the chaining
+    on the host, the grouped stack written by one pass (sdb_stack_group_remap)"""
+    import torch
+    from . import _lib as L
+    lib = L.require_cuda()
+    T = int(stack.shape[0]); S = stack.numel() // T
+    ids, offsets = stack_labels_device(stack)
+    tables = stack_overlap_device(stack, ids, offsets)
+    per_frame = [ids[offsets[f]:offsets[f + 1]] for f in range(T)]
+
+    def overlap(p):
+        a, b, c = tables[p]
+        m = np.zeros((1 + len(per_frame[p]), 1 + len(per_frame[p + 1])), np.int64)
+        m[a, b] = c
+        return m
+
+    luts = _group_chain(per_frame, overlap, thresh, criterion)
+    lut_d = torch.from_numpy(np.concatenate(luts).astype(np.int32)).cuda()
+    ids_d = torch.from_numpy(np.ascontiguousarray(ids, np.int32)).cuda()
+    off_d = torch.from_numpy(offsets).cuda()
+    out = torch.empty_like(stack)
+    L.check(lib.sdb_stack_group_remap(L.ptr(stack), T, S, L.ptr(ids_d), L.ptr(off_d), L.ptr(lut_d), L.ptr(out), L.stream_ptr()))
+    return out
