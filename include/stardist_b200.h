@@ -268,6 +268,37 @@ int sdb_mt_normal(const unsigned* h_key, int pos, int has_gauss, double gauss, l
 int sdb_augment_batch(const long long* d_params, int ndim, int batch, const int* patch_size, int n_channels, const int* grid,
                       const float* d_x, const int* d_y_raw, const int* d_y_slots, const double* d_noise, float* d_x_out,
                       int* d_y_clamped, int* d_y_slots_out, int* d_y_slots_grid, unsigned char* d_neg, sdb_stream_t stream);
+/* helpers.cu: the public helpers that read a whole label, mask or distance map (DESIGN.md §4).
+ * sdb_label_class_map: mask_to_categorical (stardist/utils.py:318-380) of an int32 label map of n pixels -> d_out float32
+ *   [n][n_classes + 1]: 0 -> channel 0 is 1; a label -> its code in d_codes at its position in the ascending d_keys [n_keys]
+ *   (every non-zero label of the map must be there): 1..n_classes one-hot, 0 all zeros, -1 (None) channel 0 is 0 and the
+ *   others -1.  Asynchronous.
+ * sdb_mask_compact_count / _write: the set elements of the box [lo, hi) of a contiguous mask d_mask [shape] (ndim in [1, 4],
+ *   elements of elem_size bytes), in C order.  An element is set when the low bit of its first byte is (nonzero 0: numpy's
+ *   mask & 1 on a bool or integer mask) or when any of its bytes is non-zero (nonzero 1: np.where).  _count writes the row
+ *   prefix d_prefix int64 [rows + 1] (rows: the box's extents over every axis but the last, multiplied) and *h_n, after one
+ *   stream synchronisation; _write then writes the n absolute coordinates axis after axis, d_coords int32 [ndim][n], and, when
+ *   d_prob (float32, the mask's shape) is not NULL, d_w [n] = d_prob at them.  Asynchronous.
+ * sdb_gather_patches: n_samples crops of shape patch [ndim] (ndim in [1, 4]) of the contiguous array d_src [shape] with
+ *   elements of elem_size in {1, 2, 4, 8, 16} bytes, starting at d_starts int64 [n_samples][ndim] -> d_out [n_samples][patch],
+ *   copied as words.  Asynchronous.
+ * sdb_dist_to_volume / sdb_dist_to_centroid: c_dist_to_volume / c_dist_to_centroid (stardist3d.cpp:146-234) on a float32 map
+ *   d_dist [nz][ny][nx][n_rays] with the rays' d_verts float32 [n_rays][3] and d_faces int32 [n_faces][3] (indices below
+ *   n_rays), n_rays <= 256, n_faces <= 512: d_out float32 [nz][ny][nx] (volume) or [nz][ny][nx][3] (centroid, plus the
+ *   voxel's (k, j, i) when absolute), bit-identical to the reference.  Asynchronous. */
+int sdb_label_class_map(const int* d_labels, long long n, const int* d_keys, const int* d_codes, int n_keys, int n_classes,
+                        float* d_out, sdb_stream_t stream);
+int sdb_mask_compact_count(const void* d_mask, int elem_size, int nonzero, int ndim, const long long* shape, const long long* lo,
+                           const long long* hi, long long* d_prefix, long long* h_n, sdb_stream_t stream);
+int sdb_mask_compact_write(const void* d_mask, int elem_size, int nonzero, int ndim, const long long* shape, const long long* lo,
+                           const long long* hi, const long long* d_prefix, long long n, int* d_coords, const float* d_prob,
+                           float* d_w, sdb_stream_t stream);
+int sdb_gather_patches(const void* d_src, int elem_size, int ndim, const long long* shape, const long long* patch,
+                       const long long* d_starts, long long n_samples, void* d_out, sdb_stream_t stream);
+int sdb_dist_to_volume(const float* d_dist, int nz, int ny, int nx, int n_rays, const float* d_verts, const int* d_faces,
+                       int n_faces, float* d_out, sdb_stream_t stream);
+int sdb_dist_to_centroid(const float* d_dist, int nz, int ny, int nx, int n_rays, const float* d_verts, const int* d_faces,
+                         int n_faces, int absolute, float* d_out, sdb_stream_t stream);
 /* host-pointer versions on any int32 label map (negative labels are never an object; relabelling, the constant-image rule and
  * the mapping back to the original labels happen inside): void, on failure the result is zeroed and sdb_last_error() holds
  * the message (cleared on success) */

@@ -14,4 +14,6 @@ from .geometry import (ray_angles, dist_to_coord, polygons_to_label, polygons_to
 from .rays3d import Rays_GoldenSpiral, Rays_Explicit, Rays_Cartesian, Rays_SubDivide, Rays_Tetra, Rays_Octo, rays_from_json
 from .matching import relabel_sequential
 from .models import Config2D, StarDist2D, Config3D, StarDist3D
-from .utils import normalize, calculate_extents, edt_prob, fill_label_holes
+from .utils import normalize, calculate_extents, edt_prob, fill_label_holes, sample_points
+from .sample_patches import sample_patches
+from .io.rois import export_imagej_rois

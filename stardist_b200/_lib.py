@@ -166,6 +166,20 @@ def _declare(lib):
     lib.sdb_mt_normal.restype = c_int
     lib.sdb_augment_batch.argtypes = [P, c_int, c_int, P, c_int, P, P, P, P, P, P, P, P, P, P, P]
     lib.sdb_augment_batch.restype = c_int
+    lib.sdb_label_class_map.argtypes = [P, c_longlong, P, P, c_int, c_int, P, P]
+    lib.sdb_label_class_map.restype = c_int
+    lib.sdb_mask_compact_count.argtypes = [P, c_int, c_int, c_int, POINTER(c_longlong), POINTER(c_longlong), POINTER(c_longlong), P,
+                                           POINTER(c_longlong), P]
+    lib.sdb_mask_compact_count.restype = c_int
+    lib.sdb_mask_compact_write.argtypes = [P, c_int, c_int, c_int, POINTER(c_longlong), POINTER(c_longlong), POINTER(c_longlong), P,
+                                           c_longlong, P, P, P, P]
+    lib.sdb_mask_compact_write.restype = c_int
+    lib.sdb_gather_patches.argtypes = [P, c_int, c_int, POINTER(c_longlong), POINTER(c_longlong), P, c_longlong, P, P]
+    lib.sdb_gather_patches.restype = c_int
+    lib.sdb_dist_to_volume.argtypes = [P, c_int, c_int, c_int, c_int, P, P, c_int, P, P]
+    lib.sdb_dist_to_volume.restype = c_int
+    lib.sdb_dist_to_centroid.argtypes = [P, c_int, c_int, c_int, c_int, P, P, c_int, c_int, P, P]
+    lib.sdb_dist_to_centroid.restype = c_int
     lib.sdb_fill_label_holes.argtypes = [P, c_int, P, c_int, c_int, P, P]
     lib.sdb_fill_label_holes.restype = c_int
     lib._LIB_edt_prob.argtypes = [P, c_int, P, P, P]
@@ -274,6 +288,10 @@ def stream_ptr(stream=None):
 
 def iarr(vals):
     return (c_int * len(vals))(*[int(v) for v in vals])
+
+
+def larr(vals):
+    return (c_longlong * len(vals))(*[int(v) for v in vals])
 
 
 def nms2d_set_filter(mode):

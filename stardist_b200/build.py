@@ -12,7 +12,7 @@ UNITS = [
     ("runtime.cu", False), ("candidates.cu", True), ("nms2d.cu", True), ("nms2d_nv32.cu", True),
     ("nms2d_nv128.cu", True), ("label2d.cu", True), ("label3d.cu", True), ("blocks.cu", True), ("prep.cu", True), ("nms3d.cu", True), ("unet_simt.cu", False), ("unet_tc.cu", False), ("unet_exec.cu", False), ("overlap.cu", False),
     ("stardist.cu", True), ("labelprep.cu", True), ("traindata.cu", True),
-    ("unet_train.cu", False), ("unet_any.cu", False), ("augment.cu", True),
+    ("unet_train.cu", False), ("unet_any.cu", False), ("augment.cu", True), ("helpers.cu", True),
 ]
 
 def _deps(src):

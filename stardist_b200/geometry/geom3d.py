@@ -1,13 +1,15 @@
 """3D geometry of the prediction path, device backed.
 
-Mirrors stardist/geometry/geom3d.py: polyhedron_to_label (:100-198), dist_to_coord3D (:261-275).
+Mirrors stardist/geometry/geom3d.py: polyhedron_to_label (:100-198), dist_to_volume / dist_to_centroid (:220-258),
+dist_to_coord3D (:261-275).
 """
 import numpy as np
-from ..utils import _normalize_grid
+from ..utils import _normalize_grid, _raise
 from .distances import star_dist3D_device, label_map_to_device, centroids_device, check_points_in, output_shape
 
 
 RENDER_MODES = ("full", "kernel", "hull", "bbox", "debug")      # index = render_mode of the C entry point
+SD3_MAX_RAYS, SD3_MAX_FACES = 256, 512                           # the 3-D kernels' limits (csrc/nms3d_pair.cuh)
 
 
 def _as_rows(a, what):
@@ -128,3 +130,68 @@ def relabel_image_stardist3D(lbl, rays, verbose=False, **kwargs):
     L.check(lib.sdb_polyhedron_to_label(L.ptr(dist), L.ptr(pts), L.ptr(verts), L.ptr(faces), n, len(rays), len(rays.faces),
                                         L.ptr(labels), nz, ny, nx, RENDER_MODES.index("full"), 0, 0, L.ptr(out), L.stream_ptr()))
     return out.cpu().numpy()
+
+
+def _dist_to_poly(dist, rays, absolute=None):
+    """sdb_dist_to_volume (absolute None) / sdb_dist_to_centroid on a float32 map [nz, ny, nx, n_rays] (numpy or CUDA)"""
+    import torch
+    from .. import _lib as L
+    verts = np.ascontiguousarray(rays.vertices, np.float32)
+    faces = np.ascontiguousarray(rays.faces, np.int32)
+    if len(verts) > SD3_MAX_RAYS or len(faces) > SD3_MAX_FACES:
+        raise ValueError("rays with %d vertices and %d faces: at most %d rays and %d faces are supported"
+                         % (len(verts), len(faces), SD3_MAX_RAYS, SD3_MAX_FACES))
+    if faces.size and (faces.min() < 0 or faces.max() >= len(verts)):
+        raise ValueError("rays.faces must index rays.vertices")
+    if isinstance(dist, torch.Tensor):
+        if not (dist.is_cuda and dist.dtype == torch.float32):
+            raise ValueError("a tensor dist must be a CUDA float32 tensor")
+        d_dist = dist.contiguous()
+    lib = L.require_cuda()
+    if not isinstance(dist, torch.Tensor):
+        d_dist = torch.from_numpy(dist).cuda()
+    nz, ny, nx, n_rays = (int(s) for s in d_dist.shape)
+    d_verts, d_faces = torch.from_numpy(verts).cuda(), torch.from_numpy(faces).cuda()
+    out = torch.empty((nz, ny, nx) + (() if absolute is None else (3,)), dtype=torch.float32, device=d_dist.device)
+    if absolute is None:
+        L.check(lib.sdb_dist_to_volume(L.ptr(d_dist), nz, ny, nx, n_rays, L.ptr(d_verts), L.ptr(d_faces), len(faces), L.ptr(out),
+                                       L.stream_ptr()))
+    else:
+        L.check(lib.sdb_dist_to_centroid(L.ptr(d_dist), nz, ny, nx, n_rays, L.ptr(d_verts), L.ptr(d_faces), len(faces),
+                                         int(absolute), L.ptr(out), L.stream_ptr()))
+    return out if isinstance(dist, torch.Tensor) else out.cpu().numpy()
+
+
+def dist_to_volume(dist, rays):
+    """ returns areas of polyhedra
+        dist.shape = (nz,ny,nx,nrays)
+
+    The volume of the star-convex polyhedron of every voxel (stardist/geometry/geom3d.py:220-236 over c_dist_to_volume),
+    float32 (nz, ny, nx), bit-identical to the reference; one device thread per voxel (helpers.cu).  dist may be a CUDA
+    float32 tensor, which gives a CUDA tensor.  At most 256 rays / 512 faces (ValueError)."""
+    import torch
+    if not isinstance(dist, torch.Tensor):
+        dist = np.asanyarray(dist)
+    dist.ndim == 4 or _raise(ValueError("dist.ndim = {dist.ndim} but should be 4".format(dist = dist)))
+    dist.shape[-1]== len(rays) or _raise(ValueError("dist.shape[-1] = {d} but should be {l}".format(d = dist.shape[-1], l = len(rays))))
+    if not isinstance(dist, torch.Tensor):
+        dist = np.ascontiguousarray(dist.astype(np.float32, copy=False))
+    return _dist_to_poly(dist, rays)
+
+
+def dist_to_centroid(dist, rays, mode='absolute'):
+    """ returns centroids of polyhedra
+
+        dist.shape = (nz,ny,nx,nrays)
+        mode = 'absolute' or 'relative'
+
+    float32 (nz, ny, nx, 3) (stardist/geometry/geom3d.py:239-258 over c_dist_to_centroid), bit-identical to the reference;
+    with mode 'absolute' the voxel's (z, y, x) is added.  dist may be a CUDA float32 tensor, which gives a CUDA tensor."""
+    import torch
+    dist.ndim == 4 or _raise(ValueError("dist.ndim = {dist.ndim} but should be 4".format(dist = dist)))
+    dist.shape[-1]== len(rays) or _raise(ValueError("dist.shape[-1] = {d} but should be {l}".format(d = dist.shape[-1], l = len(rays))))
+    if not isinstance(dist, torch.Tensor):
+        dist = np.ascontiguousarray(dist.astype(np.float32, copy=False))
+
+    mode in ('absolute', 'relative') or _raise(ValueError("mode should be either 'absolute' or 'relative'"))
+    return _dist_to_poly(dist, rays, absolute=(mode == 'absolute'))

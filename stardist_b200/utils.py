@@ -180,3 +180,160 @@ def grid_divisible_patch_size(patch_size, grid, warn=True):
     if patch_size != patch_size_divisible and warn:
         warnings.warn(f"increasing patch_size from {patch_size} to {patch_size_divisible}, since it was not evenly divisible by grid {grid}")
     return patch_size_divisible
+
+
+def _invert_dict(d):
+    """ return  v-> [k_1,k_2,k_3....] for k,v in d"""
+    from collections import defaultdict
+    res = defaultdict(list)
+    for k, v in d.items():
+        res[v].append(k)
+    return res
+
+
+_INT32_MAX = int(np.iinfo(np.int32).max)
+
+
+def _class_code(cls, n_classes):
+    """the class-map code of one class id (stardist/utils.py:365-372): -1 for None, else the id in 0..n_classes"""
+    if cls is None:
+        return -1
+    if np.issubdtype(type(cls), np.integer) and 0 <= cls <= n_classes:
+        return int(cls)
+    raise ValueError(f"Wrong class id '{cls}' (for n_classes={n_classes})")
+
+
+def mask_to_categorical(y, n_classes, classes, return_cls_dict=False):
+    """generates a multi-channel categorical class map (stardist/utils.py:318-380)
+
+    y: integer label array (labels below 2^31), or a contiguous CUDA int32 tensor; n_classes: number of object classes
+    (without background); classes: dict {label -> class_id} with class_id 0 (background), 1..n_classes or None (ignored
+    object: -1 in the object channels), or a single integer / None broadcast to every label of y.
+
+    Returns the probability map float32 y.shape + (n_classes + 1,) (first channel is background), as numpy for numpy input
+    and as a CUDA tensor for a CUDA tensor, and with return_cls_dict also the inverted dict {class_id -> [labels]}.
+    The labels of y are found on the device (sdb_stack_labels), only their id list comes back to be checked against the
+    dict, and one pass writes the map (sdb_label_class_map).  A dict's class ids are checked before the device is used, so a
+    dict with both a wrong class id and a missing label reports the class id."""
+    import torch
+    from . import _lib as L
+    from .matching import _check_label_array, stack_labels_device
+    is_tensor = isinstance(y, torch.Tensor)
+    if is_tensor:
+        if not (y.is_cuda and y.dtype == torch.int32 and y.is_contiguous()):
+            raise ValueError("mask_to_categorical expects a contiguous CUDA int32 tensor (or a numpy label array)")
+    else:
+        _check_label_array(y, 'y')
+        if np.iinfo(y.dtype).max > _INT32_MAX and y.size and int(y.max()) > _INT32_MAX:
+            raise ValueError("mask_to_categorical: labels must be below 2^31")
+    if not (np.issubdtype(type(n_classes), np.integer) and n_classes >= 1):
+        raise ValueError(f"n_classes is '{n_classes}' but should be a positive integer")
+    broadcast = np.issubdtype(type(classes), np.integer) or classes is None
+    if not (broadcast or isinstance(classes, dict)):
+        raise ValueError("classes should be dict, single scalar, or None!")
+    if not broadcast:
+        for cls in _invert_dict(classes):
+            _class_code(cls, n_classes)
+
+    lib = L.require_cuda()
+    shape = tuple(y.shape)
+    d_y = y if is_tensor else torch.from_numpy(np.ascontiguousarray(y, dtype=np.int32)).cuda()
+    try:
+        ids, _ = stack_labels_device(d_y.reshape(1, -1))
+    except ValueError:
+        raise ValueError("y must be an array of non-negative integers.")
+    y_labels = ids.tolist()
+    if broadcast:
+        classes = dict((k, classes) for k in y_labels)
+    if not set(y_labels).issubset(set(classes.keys())):
+        raise ValueError(f"all gt labels should be present in class dict provided \ngt_labels found\n{set(y_labels)}\nclass dict labels provided\n{set(classes.keys())}")
+    cls_dict = _invert_dict(classes)
+    for cls in cls_dict:
+        _class_code(cls, n_classes)
+
+    codes = np.array([_class_code(classes[k], n_classes) for k in y_labels], np.int32)
+    d_keys = torch.from_numpy(np.ascontiguousarray(ids, np.int32)).cuda()
+    d_codes = torch.from_numpy(codes).cuda()
+    out = torch.empty(shape + (n_classes + 1,), dtype=torch.float32, device=d_y.device)
+    L.check(lib.sdb_label_class_map(L.ptr(d_y), d_y.numel(), L.ptr(d_keys), L.ptr(d_codes), len(y_labels), int(n_classes),
+                                    L.ptr(out), L.stream_ptr()))
+    y_mask = out if is_tensor else out.cpu().numpy()
+    return (y_mask, cls_dict) if return_cls_dict else y_mask
+
+
+def _mask_compact_device(mask, nonzero, lo, hi, prob=None):
+    """The set elements of the box [lo, hi) of a mask (numpy array or CUDA tensor of bool / integers, at most 4-D), in C order,
+    compacted on the device (sdb_mask_compact_count / _write): a tuple of int32 host coordinate arrays, one per axis, and the
+    float32 values of `prob` (a CUDA float32 tensor of the mask's shape, or None) at them.  nonzero: an element is set when it
+    is non-zero (np.where), else when its low bit is (numpy's mask & 1)."""
+    import ctypes, torch
+    from . import _lib as L
+    lib = L.require_cuda()
+    if isinstance(mask, torch.Tensor):
+        d_m = mask.contiguous()
+        elem = d_m.element_size()
+    else:
+        m = np.ascontiguousarray(mask)
+        elem = m.itemsize
+        d_m = torch.from_numpy(m.view(np.uint8).reshape(-1)).cuda()
+    ndim, shape = len(lo), tuple(int(s) for s in mask.shape)
+    rows = int(np.prod([max(0, h - l) for l, h in zip(lo[:-1], hi[:-1])], dtype=np.int64))
+    pre = torch.empty(rows + 1, dtype=torch.int64, device='cuda')
+    args = (L.ptr(d_m), elem, int(bool(nonzero)), ndim, L.larr(shape), L.larr(lo), L.larr(hi))
+    h_n = ctypes.c_longlong(0)
+    L.check(lib.sdb_mask_compact_count(*args, L.ptr(pre), ctypes.byref(h_n), L.stream_ptr()))
+    n = int(h_n.value)
+    coords = torch.empty((ndim, n), dtype=torch.int32, device='cuda')
+    w = torch.empty(n, dtype=torch.float32, device='cuda') if prob is not None else None
+    L.check(lib.sdb_mask_compact_write(*args, L.ptr(pre), n, L.ptr(coords), L.ptr(prob), L.ptr(w), L.stream_ptr()))
+    return tuple(coords.cpu().numpy()), (None if w is None else w.cpu().numpy())
+
+
+def sample_points(n_samples, mask, prob=None, b=2):
+    """sample points to draw some of the associated polygons (stardist/utils.py:156-177)
+
+    Candidates are the set pixels of `mask & 1` (a 2-D bool or integer mask) at least `b` pixels inside the border (every
+    pixel for b None or 0), in C order; they are drawn with np.random.choice(n, n_samples, replace=True), weighted by `prob`
+    at the candidates when it is given.  Returns int64 [n_samples, 2] (y, x).
+
+    The candidates are compacted on the device, which also gathers `prob` there when it is a CUDA float32 tensor (a numpy
+    `prob` is read on the host at the candidates); the mask may be a numpy array or a CUDA bool / integer tensor, e.g. from a
+    device-resident predict.  The draw makes the reference's numpy calls on the candidates, so points and np.random's state
+    are the reference's.  Deliberate difference: a mask that is not 2-D raises ValueError."""
+    import torch
+    is_tensor = isinstance(mask, torch.Tensor)
+    use_border = b is not None and b > 0
+    if is_tensor:
+        if not mask.is_cuda or mask.dtype.is_floating_point or mask.dtype.is_complex:
+            raise TypeError("sample_points: a tensor mask must be a CUDA bool or integer tensor")
+    else:
+        mask = np.asanyarray(mask)
+        if not (mask.dtype == bool or np.issubdtype(mask.dtype, np.integer)):
+            empty = np.zeros(0, mask.dtype)
+            empty & (empty if use_border else True)                         # numpy's own TypeError
+    if mask.ndim != 2:
+        raise ValueError("sample_points: mask must be 2-dimensional (it has %d dimensions)" % mask.ndim)
+    shape = tuple(int(s) for s in mask.shape)
+    if use_border:
+        box = [slice(b, -b).indices(s)[:2] for s in shape]                  # mask_b[b:-b, b:-b] = True
+    else:
+        box = [(0, s) for s in shape]
+    lo, hi = [l for l, _ in box], [max(l, h) for l, h in box]
+    d_prob = prob if isinstance(prob, torch.Tensor) else None
+    if d_prob is not None and not (d_prob.is_cuda and d_prob.dtype == torch.float32 and tuple(d_prob.shape) == shape):
+        raise ValueError("sample_points: a tensor prob must be a CUDA float32 tensor of the mask's shape")
+    points, w = _mask_compact_device(mask, False, lo, hi, None if d_prob is None else d_prob.contiguous())
+    points = tuple(p.astype(np.intp) for p in points)
+
+    if prob is not None:
+        # weighted sampling via prob
+        w = (w if d_prob is not None else prob[points[0], points[1]]).astype(np.float64)
+        w /= np.sum(w)
+        ind = np.random.choice(len(points[0]), n_samples, replace=True, p=w)
+    else:
+        ind = np.random.choice(len(points[0]), n_samples, replace=True)
+
+    points = points[0][ind], points[1][ind]
+    points = np.stack(points, axis=-1)
+    return points
+
