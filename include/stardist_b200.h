@@ -498,6 +498,19 @@ int sdb_conv_wgrad_any_nd(const float* d_x, const float* d_x_lo, int n, int d, i
  * gradient of a stride-1 3^d 'same' convolution is sdb_conv3_nd of dy with wf, zero bias, no ReLU (sdb_conv_dgrad_any_nd
  * for other extents) */
 int sdb_conv_flip_weights(const float* d_w, int taps, int cin, int cout, float* d_wf, sdb_stream_t stream);
+/* TF32 tensor-core variants of the two gradients above (csrc/unet_train_tf32.cu), the precision mode of
+ * stardist_b200.enable_tensor_float_32_execution (DESIGN.md 4.2).  rna(v) is cvt.rna.tf32.f32: v rounded to 10 explicit
+ * mantissa bits, nearest, ties away from zero; products accumulate in fp32, with no float atomics (bit-identical run to run).
+ * sdb_conv_wgrad_tf32_nd: sdb_conv_wgrad_nd's arguments, shapes and workspace; dw = sum_p rna(x[p + tap]) * rna(dy[p]) and
+ * db = sum_p dy[p] unrounded, in fp32.  sdb_conv_dgrad_tf32_nd: the input gradient of a stride-1 3^d 'same' convolution,
+ * gin [n,d,h,w,cin] = sum over (tap, co) of rna(dy[p + tap - 1, co]) * rna(wf[tap, co, ci]) with wf (k..., cout, cin) from
+ * sdb_conv_flip_weights (kz = 1 with d = 1 in 2-D, kz = 3 in 3-D; kyx = 3); the shapes sdb_conv3_nd takes for it: cout <= 4
+ * with cin 32 or 64, or cout % 8 == 0 with cin % 32 == 0. */
+int sdb_conv_wgrad_tf32_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                           int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
+                           long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
+int sdb_conv_dgrad_tf32_nd(const float* d_dy, int n, int d, int h, int w, int cout, const float* d_wf, int cin, int kz, int kyx,
+                           float* d_gin, sdb_stream_t stream);
 /* gradient of [upsample(x_lo), skip] -> d x_lo (block sums, the backward of nearest up-sampling) and d skip (overwritten) */
 int sdb_decoder_split(const float* d_dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy, int ux,
                       float* d_dlo, float* d_dskip, sdb_stream_t stream);

@@ -71,6 +71,10 @@ def _declare(lib):
     lib.sdb_conv_wgrad_workspace.restype = c_longlong
     lib.sdb_conv_wgrad_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, P, c_longlong, P, P, P]
     lib.sdb_conv_wgrad_nd.restype = c_int
+    lib.sdb_conv_wgrad_tf32_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, P, c_longlong, P, P, P]
+    lib.sdb_conv_wgrad_tf32_nd.restype = c_int
+    lib.sdb_conv_dgrad_tf32_nd.argtypes = [P] + [c_int] * 5 + [P] + [c_int] * 3 + [P, P]
+    lib.sdb_conv_dgrad_tf32_nd.restype = c_int
     lib.sdb_conv_wgrad_any_nd.argtypes = [P, P] + [c_int] * 12 + [P, c_int, c_int, P, c_longlong, P, P, P]
     lib.sdb_conv_wgrad_any_nd.restype = c_int
     lib.sdb_conv_dgrad_any_nd.argtypes = [P] + [c_int] * 5 + [P] + [c_int] * 4 + [P, P]

@@ -12,6 +12,7 @@
 #include <string>
 #include <algorithm>
 #include "common.cuh"
+#include "wgrad.cuh"
 #include "../../include/stardist_b200.h"
 
 namespace {
@@ -30,13 +31,7 @@ __device__ __forceinline__ long long llmin(long long a, long long b) { return a 
 // the pixel range writes work[s][row][co].
 constexpr int WG_R = 64, WG_C = 64, WG_K = 16;
 
-struct WgradArgs {
-  const float* x; const float* x_lo; const float* dy;
-  int n, d, h, w, c_skip, c_lo, uz, uy, ux, kz, ky, kx, pz, py, px, ldy, cout;
-  int rows;                 // taps * Cin + 1
-  long long npix, per_split;
-  float* work;
-};
+using sdb::WgradArgs;
 
 __global__ void __launch_bounds__(256) k_conv_wgrad(WgradArgs A) {
   __shared__ __align__(16) float sX[WG_K][WG_R];
@@ -466,9 +461,10 @@ extern "C" long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin,
 
 namespace {
 
+// tf32 = true runs the partial sums on the TF32 tensor cores (unet_train_tf32.cu) over the same splits and workspace
 int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
                int uz, int uy, int ux, int kz, int ky, int kx, const float* d_dy, int ldy, int cout, float* d_work,
-               long long work_floats, float* d_dw, float* d_db, cudaStream_t st) {
+               long long work_floats, float* d_dw, float* d_db, cudaStream_t st, bool tf32 = false) {
   if (n < 1 || d < 1 || h < 1 || w < 1 || cout < 1 || ldy < cout || cin_skip < 0 || cin_lo < 0 || cin_skip + cin_lo < 1) {
     sdb::set_error(std::string(who) + ": bad arguments"); return 1;
   }
@@ -487,8 +483,12 @@ int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, in
   const int ns = wgrad_split(A.npix, A.rows, cout, &A.per_split);
   if ((long long)ns * A.rows * cout > work_floats) { sdb::set_error(std::string(who) + ": workspace too small"); return 1; }
   A.work = d_work;
-  dim3 grid(cdiv(A.rows, WG_R) * cdiv(cout, WG_C), ns);
-  SDB_LAUNCH(k_conv_wgrad, grid, 256, 0, st, A);
+  if (tf32) {
+    if (sdb::conv_wgrad_tf32_launch(A, ns, st)) return 1;
+  } else {
+    dim3 grid(cdiv(A.rows, WG_R) * cdiv(cout, WG_C), ns);
+    SDB_LAUNCH(k_conv_wgrad, grid, 256, 0, st, A);
+  }
   SDB_LAUNCH(k_wgrad_reduce, grid_1d((long long)A.rows * cout, 16), 256, 0, st, d_work, ns, A.rows, cout, d_dw, d_db);
   return 0;
 }
@@ -501,6 +501,14 @@ extern "C" int sdb_conv_wgrad_nd(const float* d_x, const float* d_x_lo, int n, i
   if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_nd: kernel must be 1^d or 3^d"); return 1; }
   return conv_wgrad("conv_wgrad_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, kyx, kyx, d_dy, ldy, cout, d_work,
                     work_floats, d_dw, d_db, (cudaStream_t)stream);
+}
+
+extern "C" int sdb_conv_wgrad_tf32_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                                      int uz, int uy, int ux, int kz, int kyx, const float* d_dy, int ldy, int cout, float* d_work,
+                                      long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
+  if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_tf32_nd: kernel must be 1^d or 3^d"); return 1; }
+  return conv_wgrad("conv_wgrad_tf32_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, kyx, kyx, d_dy, ldy, cout, d_work,
+                    work_floats, d_dw, d_db, (cudaStream_t)stream, true);
 }
 
 extern "C" int sdb_conv_wgrad_any_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,

@@ -13,6 +13,23 @@ from ..utils import _raise
 
 ADAM_BETA_1, ADAM_BETA_2, ADAM_EPSILON = 0.9, 0.999, 1e-7     # tf.keras.optimizers.Adam defaults
 
+_tensor_float_32 = False
+
+
+def enable_tensor_float_32_execution(enabled):
+    """TensorFlow's tf.config.experimental.enable_tensor_float_32_execution for training: when on, the weight gradients of the
+    1^d / 3^d / (1, 3, 3) convolutions and the input gradients of the 3^d ones run on the TF32 tensor cores (operands rounded to
+    10 mantissa bits, fp32 accumulation; DESIGN.md 4.2).  Off by default, unlike TensorFlow: the backward pass is then exact
+    fp32.  The forward pass, the loss and prediction never change.  A UNetTrainer (and so train()) reads the switch once,
+    when it is constructed."""
+    global _tensor_float_32
+    _tensor_float_32 = bool(enabled)
+
+
+def tensor_float_32_execution_enabled():
+    """whether trainers constructed from now on run their convolution gradients in TF32"""
+    return _tensor_float_32
+
 
 def check_trainable(config, optimizer=None):
     """NotImplementedError for every setting this trainer does not cover; runs before anything touches the device"""
@@ -57,6 +74,7 @@ class UNetTrainer:
         from .unet_device import UNetDeviceND
         check_trainable(config)
         lib = L.require_cuda()
+        self.tf32 = tensor_float_32_execution_enabled()
         self.config, self.nd = config, config.n_dim
         self.net = UNetDeviceND(config, weights)
         self.layers = self.net.layers
@@ -127,8 +145,9 @@ class UNetTrainer:
         need = int(lib.sdb_conv_wgrad_workspace(n * d * h * w, kz * ky * kx, c_skip + c_lo, cout))
         work = self._workspace(need)
         if conv_wgrad_accepts(self.nd, k):
-            L.check(lib.sdb_conv_wgrad_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, L.ptr(dy), ldy,
-                                          cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
+            wgrad = lib.sdb_conv_wgrad_tf32_nd if self.tf32 else lib.sdb_conv_wgrad_nd
+            L.check(wgrad(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, L.ptr(dy), ldy,
+                          cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
         else:
             L.check(lib.sdb_conv_wgrad_any_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, kx, L.ptr(dy),
                                               ldy, cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
@@ -159,7 +178,8 @@ class UNetTrainer:
 
     def _dgrad(self, key, name, g, x_shape, cin, cout, k):
         """input gradient of the stride-1 convolution `name` (kernel extents k, x_shape [..., cin] -> cout): the correlation of g
-        with the flipped kernel, on sdb_conv3_nd where conv_dgrad3_accepts takes the layer, else on sdb_conv_dgrad_any_nd"""
+        with the flipped kernel, on sdb_conv3_nd (sdb_conv_dgrad_tf32_nd in TF32 mode) where conv_dgrad3_accepts takes the layer,
+        else on sdb_conv_dgrad_any_nd"""
         from .unet_device import conv_dgrad3_accepts
         lib = L.load()
         st = L.stream_ptr()
@@ -168,7 +188,9 @@ class UNetTrainer:
         L.check(lib.sdb_conv_flip_weights(L.ptr(self.pview[name][0]), taps, cin, cout, L.ptr(wf), st))
         n = x_shape[0]; d, h, w = (1,) + tuple(x_shape[1:3]) if len(x_shape) == 4 else tuple(x_shape[1:4])
         gin = self._buf(('gin', key), tuple(x_shape[:-1]) + (cin,))
-        if conv_dgrad3_accepts(self.nd, k, cin, cout):
+        if conv_dgrad3_accepts(self.nd, k, cin, cout) and self.tf32:
+            L.check(lib.sdb_conv_dgrad_tf32_nd(L.ptr(g), n, d, h, w, cout, L.ptr(wf), cin, 1 if self.nd == 2 else 3, 3, L.ptr(gin), st))
+        elif conv_dgrad3_accepts(self.nd, k, cin, cout):
             zb = self._buf(('zero_bias', cin), (cin,), zero=True)
             L.check(lib.sdb_conv3_nd(L.ptr(g), None, n, d, h, w, cout, 0, 1, 1, 1, L.ptr(wf), L.ptr(zb), cin,
                                      1 if self.nd == 2 else 3, 0, L.ptr(gin), st))
