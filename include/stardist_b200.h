@@ -511,6 +511,48 @@ int sdb_conv_wgrad_tf32_nd(const float* d_x, const float* d_x_lo, int n, int d, 
                            long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
 int sdb_conv_dgrad_tf32_nd(const float* d_dy, int n, int d, int h, int w, int cout, const float* d_wf, int cin, int kz, int kyx,
                            float* d_gin, sdb_stream_t stream);
+/* bf16 tensor-core training kernels (csrc/unet_train_bf16.cu), the mixed_bfloat16 policy of stardist_b200.mixed_precision
+ * (DESIGN.md 4.2).  Activations and gradients between layers are bf16 (void* below: __nv_bfloat16); parameters, biases and
+ * gradients of parameters are fp32.  Every GEMM multiplies bf16 values and accumulates in fp32; an fp32 operand is rounded
+ * to bf16 on load (round to nearest even); every bf16 store is one such rounding of an fp32 value.  No float atomics.
+ * sdb_cast_bf16: out = bf16(in).  sdb_weights_bf16: w (taps, cin, cout) fp32 -> bf16, flip = 0 to out[(tap*cout + co)*ld +
+ * ci] (the layout sdb_conv_bf16_nd reads, ld = cin), flip = 1 to out[((taps-1-tap)*cin + ci)*ld + co] (the flipped kernel
+ * of sdb_conv_flip_weights in that layout, ld = cout: the input gradient's weights).
+ * sdb_conv_bf16_nd: y = act(conv(x) + b) with 'same' padding, stride 1, extents kz, ky, kx in {1, 3}, over the input
+ * [upsample(x_lo), skip] (x = skip, cin_lo = 0 for none); wb [taps][cout][cin_skip + cin_lo] bf16, b fp32 [cout] or NULL;
+ * relu = 1 applies ReLU; accumulate = 1 adds the result to the bf16 already in d_out (one rounding of the sum).  The input
+ * gradient is this kernel on dy with the flip = 1 weights, no bias.
+ * sdb_gemm_bf16_f32in: out [npix][nout] bf16 (+)= a [npix][k] (fp32, rounded on load) . wb [nout][k] -- the heads' and class
+ * head's input gradients.  sdb_heads_bf16: prob = sigmoid(f . wp + bp), dist = f . wd + bd in fp32 from bf16 features, wb
+ * [n_rays + 1][cfeat] (row 0 the prob kernel).  sdb_class_head_bf16: softmax(f . w + b) in fp32, wb [n_out][cfeat], logits
+ * fp32 [npix][n_out] scratch.
+ * sdb_conv_wgrad_bf16_nd: sdb_conv_wgrad_nd on bf16 x, x_lo and a dy that is bf16 (dy_bf16 = 1: ldy and cout multiples of 8)
+ * or fp32 (rounded on load); kernels 1^d, 3^d and (1, 3, 3) (kz = 1, kyx = 3); same workspace and split reduction; db = sum_p
+ * dy[p] in fp32 of dy as stored.
+ * The rest are the bf16 versions of sdb_maxpool_any_nd, sdb_maxpool_backward_nd, sdb_relu_backward, sdb_decoder_split and
+ * out = bf16(a + b). */
+int sdb_cast_bf16(const float* d_in, long long n, void* d_out, sdb_stream_t stream);
+int sdb_weights_bf16(const float* d_w, int taps, int cin, int cout, int flip, int ld, void* d_out, sdb_stream_t stream);
+int sdb_conv_bf16_nd(const void* d_x, const void* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo, int uz, int uy,
+                     int ux, int kz, int ky, int kx, const void* d_wb, const float* d_b, int cout, int relu, int accumulate,
+                     void* d_out, sdb_stream_t stream);
+int sdb_gemm_bf16_f32in(const float* d_a, long long npix, int k, const void* d_wb, int nout, int accumulate, void* d_out,
+                        sdb_stream_t stream);
+int sdb_heads_bf16(const void* d_feat, long long npix, int cfeat, const void* d_wb, const float* d_bp, const float* d_bd,
+                   int n_rays, float* d_prob, float* d_dist, sdb_stream_t stream);
+int sdb_class_head_bf16(const void* d_feat, long long npix, int cfeat, const void* d_wb, const float* d_b, int n_out,
+                        float* d_logits, float* d_out, sdb_stream_t stream);
+int sdb_conv_wgrad_bf16_nd(const void* d_x, const void* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                           int uz, int uy, int ux, int kz, int kyx, const void* d_dy, int dy_bf16, int ldy, int cout,
+                           float* d_work, long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream);
+int sdb_maxpool_bf16_nd(const void* d_in, int n, int d, int h, int w, int c, int pz, int py, int px, void* d_out,
+                        sdb_stream_t stream);
+int sdb_maxpool_backward_bf16_nd(const void* d_x, const void* d_gy, int n, int d, int h, int w, int c, int pz, int py, int px,
+                                 int accumulate, void* d_gx, sdb_stream_t stream);
+int sdb_relu_backward_bf16(void* d_g, const void* d_y, long long n, sdb_stream_t stream);
+int sdb_decoder_split_bf16(const void* d_dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy, int ux,
+                           void* d_dlo, void* d_dskip, sdb_stream_t stream);
+int sdb_add_bf16(const void* d_a, const void* d_b, long long n, void* d_out, sdb_stream_t stream);
 /* gradient of [upsample(x_lo), skip] -> d x_lo (block sums, the backward of nearest up-sampling) and d skip (overwritten) */
 int sdb_decoder_split(const float* d_dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy, int ux,
                       float* d_dlo, float* d_dskip, sdb_stream_t stream);

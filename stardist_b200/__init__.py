@@ -15,6 +15,7 @@ from .rays3d import Rays_GoldenSpiral, Rays_Explicit, Rays_Cartesian, Rays_SubDi
 from .matching import relabel_sequential
 from .models import Config2D, StarDist2D, Config3D, StarDist3D
 from .models.train import enable_tensor_float_32_execution, tensor_float_32_execution_enabled
+from . import mixed_precision
 from .utils import normalize, calculate_extents, edt_prob, fill_label_holes, sample_points
 from .sample_patches import sample_patches
 from .io.rois import export_imagej_rois

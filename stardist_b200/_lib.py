@@ -75,6 +75,30 @@ def _declare(lib):
     lib.sdb_conv_wgrad_tf32_nd.restype = c_int
     lib.sdb_conv_dgrad_tf32_nd.argtypes = [P] + [c_int] * 5 + [P] + [c_int] * 3 + [P, P]
     lib.sdb_conv_dgrad_tf32_nd.restype = c_int
+    lib.sdb_cast_bf16.argtypes = [P, c_longlong, P, P]
+    lib.sdb_cast_bf16.restype = c_int
+    lib.sdb_weights_bf16.argtypes = [P] + [c_int] * 5 + [P, P]
+    lib.sdb_weights_bf16.restype = c_int
+    lib.sdb_conv_bf16_nd.argtypes = [P, P] + [c_int] * 12 + [P, P, c_int, c_int, c_int, P, P]
+    lib.sdb_conv_bf16_nd.restype = c_int
+    lib.sdb_gemm_bf16_f32in.argtypes = [P, c_longlong, c_int, P, c_int, c_int, P, P]
+    lib.sdb_gemm_bf16_f32in.restype = c_int
+    lib.sdb_heads_bf16.argtypes = [P, c_longlong, c_int, P, P, P, c_int, P, P, P]
+    lib.sdb_heads_bf16.restype = c_int
+    lib.sdb_class_head_bf16.argtypes = [P, c_longlong, c_int, P, P, c_int, P, P, P]
+    lib.sdb_class_head_bf16.restype = c_int
+    lib.sdb_conv_wgrad_bf16_nd.argtypes = [P, P] + [c_int] * 11 + [P, c_int, c_int, c_int, P, c_longlong, P, P, P]
+    lib.sdb_conv_wgrad_bf16_nd.restype = c_int
+    lib.sdb_maxpool_bf16_nd.argtypes = [P] + [c_int] * 8 + [P, P]
+    lib.sdb_maxpool_bf16_nd.restype = c_int
+    lib.sdb_maxpool_backward_bf16_nd.argtypes = [P, P] + [c_int] * 9 + [P, P]
+    lib.sdb_maxpool_backward_bf16_nd.restype = c_int
+    lib.sdb_relu_backward_bf16.argtypes = [P, P, c_longlong, P]
+    lib.sdb_relu_backward_bf16.restype = c_int
+    lib.sdb_decoder_split_bf16.argtypes = [P] + [c_int] * 9 + [P, P, P]
+    lib.sdb_decoder_split_bf16.restype = c_int
+    lib.sdb_add_bf16.argtypes = [P, P, c_longlong, P, P]
+    lib.sdb_add_bf16.restype = c_int
     lib.sdb_conv_wgrad_any_nd.argtypes = [P, P] + [c_int] * 12 + [P, c_int, c_int, P, c_longlong, P, P, P]
     lib.sdb_conv_wgrad_any_nd.restype = c_int
     lib.sdb_conv_dgrad_any_nd.argtypes = [P] + [c_int] * 5 + [P] + [c_int] * 4 + [P, P]

@@ -1,5 +1,5 @@
 // unet_train.cu -- fp32 CUDA-core kernels of the U-Net training step (NHWC / NDHWC): weight gradients of the
-// 3^d / 1^d convolutions, the decoder split, ReLU and max-pool backward, the StarDist loss with its head gradient,
+// 3^d / 1^d convolutions, the decoder split, ReLU and max-pool backward (the float instances of train_elem.cuh), the StarDist loss with its head gradient,
 // the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients and Adam.  The input gradient of the
 // convolutions is not here: it is a forward kernel run on dY with the spatially flipped, Cin/Cout-transposed kernel written by
 // sdb_conv_flip_weights -- sdb_conv3_nd of unet_simt.cu for the 3^d layers it takes, sdb_conv_dgrad_any_nd of unet_any.cu
@@ -13,6 +13,7 @@
 #include <algorithm>
 #include "common.cuh"
 #include "wgrad.cuh"
+#include "train_elem.cuh"
 #include "../../include/stardist_b200.h"
 
 namespace {
@@ -148,62 +149,6 @@ __global__ void k_flip_weights(const float* __restrict__ w, int taps, int cin, i
     const int co = (int)(e % cout); const long long r = e / cout;
     const int ci = (int)(r % cin), tap = (int)(r / cin);
     wf[((size_t)(taps - 1 - tap) * cout + co) * cin + ci] = w[e];
-  }
-}
-
-// d[up(x_lo), skip] -> d x_lo (sum over each uz*uy*ux block, row-major) and d skip (the remaining channels)
-__global__ void k_decoder_split(const float* __restrict__ dcat, int n, int d, int h, int w, int c_lo, int c_skip, int uz, int uy,
-                                int ux, float* __restrict__ dlo, float* __restrict__ dskip) {
-  const int Dl = d / uz, Hl = h / uy, Wl = w / ux, C = c_lo + c_skip;
-  const long long n_lo = (long long)n * Dl * Hl * Wl * c_lo, n_sk = (long long)n * d * h * w * c_skip;
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n_lo + n_sk; e += (long long)gridDim.x * blockDim.x) {
-    if (e < n_lo) {
-      const int c = (int)(e % c_lo); long long r = e / c_lo;
-      const int xl = (int)(r % Wl); r /= Wl;
-      const int yl = (int)(r % Hl); r /= Hl;
-      const int zl = (int)(r % Dl); const long long img = r / Dl;
-      float s = 0.f;
-      for (int a = 0; a < uz; ++a) for (int b = 0; b < uy; ++b) for (int q = 0; q < ux; ++q)
-        s += dcat[((((size_t)img * d + zl * uz + a) * h + yl * uy + b) * w + xl * ux + q) * C + c];
-      dlo[e] = s;
-    } else {
-      const long long f = e - n_lo;
-      const int c = (int)(f % c_skip); const long long p = f / c_skip;
-      dskip[f] = dcat[(size_t)p * C + c_lo + c];
-    }
-  }
-}
-
-__global__ void k_relu_backward(float* __restrict__ g, const float* __restrict__ y, long long n) {
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x)
-    if (!(y[e] > 0.f)) g[e] = 0.f;
-}
-
-// Max-pool backward: the window's gradient goes to its FIRST maximum in row-major order (TF's and torch's tie rule); the
-// other window positions receive 0.  Ties are common at 0 after a ReLU; they are harmless, because the ReLU backward of
-// the pooled tensor's producer zeroes the gradient at every position whose value is 0, whichever one got it.
-// accumulate = 1 adds to dx (a skip tensor whose decoder gradient is already there); windows do not overlap.
-__global__ void k_maxpool_backward(const float* __restrict__ x, const float* __restrict__ gy, int N, int D, int H, int W, int C,
-                                   int pz, int py, int px, int accumulate, float* __restrict__ gx) {
-  const int Do = D / pz, Ho = H / py, Wo = W / px;
-  const long long total = (long long)N * Do * Ho * Wo * C;
-  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-    const int c = (int)(e % C); long long r = e / C;
-    const int xo = (int)(r % Wo); r /= Wo;
-    const int yo = (int)(r % Ho); r /= Ho;
-    const int zo = (int)(r % Do); const long long img = r / Do;
-    float m = -INFINITY; int best = 0, k = 0;
-    for (int a = 0; a < pz; ++a) for (int b = 0; b < py; ++b) for (int q = 0; q < px; ++q, ++k) {
-      const float v = x[((((size_t)img * D + zo * pz + a) * H + yo * py + b) * W + xo * px + q) * C + c];
-      if (v > m) { m = v; best = k; }
-    }
-    const float g = gy[e];
-    k = 0;
-    for (int a = 0; a < pz; ++a) for (int b = 0; b < py; ++b) for (int q = 0; q < px; ++q, ++k) {
-      const size_t i = ((((size_t)img * D + zo * pz + a) * H + yo * py + b) * W + xo * px + q) * C + c;
-      const float v = (k == best) ? g : 0.f;
-      gx[i] = accumulate ? gx[i] + v : v;
-    }
   }
 }
 
@@ -461,10 +406,11 @@ extern "C" long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin,
 
 namespace {
 
-// tf32 = true runs the partial sums on the TF32 tensor cores (unet_train_tf32.cu) over the same splits and workspace
-int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
-               int uz, int uy, int ux, int kz, int ky, int kx, const float* d_dy, int ldy, int cout, float* d_work,
-               long long work_floats, float* d_dw, float* d_db, cudaStream_t st, bool tf32 = false) {
+// prec selects the partial-sum kernel over the same splits and workspace: WGRAD_FP32 (here), WGRAD_TF32 (the TF32 tensor
+// cores, unet_train_tf32.cu) or WGRAD_BF16_* (bf16 tensor cores on bf16 activations, unet_train_bf16.cu)
+int conv_wgrad(const char* who, const void* d_x, const void* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+               int uz, int uy, int ux, int kz, int ky, int kx, const void* d_dy, int ldy, int cout, float* d_work,
+               long long work_floats, float* d_dw, float* d_db, cudaStream_t st, int prec = sdb::WGRAD_FP32) {
   if (n < 1 || d < 1 || h < 1 || w < 1 || cout < 1 || ldy < cout || cin_skip < 0 || cin_lo < 0 || cin_skip + cin_lo < 1) {
     sdb::set_error(std::string(who) + ": bad arguments"); return 1;
   }
@@ -472,7 +418,7 @@ int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, in
     sdb::set_error(std::string(who) + ": low-resolution source needs a pointer and divisible up-sampling factors"); return 1;
   }
   WgradArgs A;
-  A.x = d_x; A.x_lo = d_x_lo; A.dy = d_dy;
+  A.x = (const float*)d_x; A.x_lo = (const float*)d_x_lo; A.dy = (const float*)d_dy; A.prec = prec;
   A.n = n; A.d = d; A.h = h; A.w = w; A.c_skip = cin_skip; A.c_lo = cin_lo;
   A.uz = cin_lo ? uz : 1; A.uy = cin_lo ? uy : 1; A.ux = cin_lo ? ux : 1;
   A.kz = kz; A.ky = ky; A.kx = kx; A.pz = (kz - 1) / 2; A.py = (ky - 1) / 2; A.px = (kx - 1) / 2;
@@ -483,8 +429,10 @@ int conv_wgrad(const char* who, const float* d_x, const float* d_x_lo, int n, in
   const int ns = wgrad_split(A.npix, A.rows, cout, &A.per_split);
   if ((long long)ns * A.rows * cout > work_floats) { sdb::set_error(std::string(who) + ": workspace too small"); return 1; }
   A.work = d_work;
-  if (tf32) {
+  if (prec == sdb::WGRAD_TF32) {
     if (sdb::conv_wgrad_tf32_launch(A, ns, st)) return 1;
+  } else if (prec != sdb::WGRAD_FP32) {
+    if (sdb::conv_wgrad_bf16_launch(A, ns, st)) return 1;
   } else {
     dim3 grid(cdiv(A.rows, WG_R) * cdiv(cout, WG_C), ns);
     SDB_LAUNCH(k_conv_wgrad, grid, 256, 0, st, A);
@@ -508,7 +456,15 @@ extern "C" int sdb_conv_wgrad_tf32_nd(const float* d_x, const float* d_x_lo, int
                                       long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
   if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_tf32_nd: kernel must be 1^d or 3^d"); return 1; }
   return conv_wgrad("conv_wgrad_tf32_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, kyx, kyx, d_dy, ldy, cout, d_work,
-                    work_floats, d_dw, d_db, (cudaStream_t)stream, true);
+                    work_floats, d_dw, d_db, (cudaStream_t)stream, sdb::WGRAD_TF32);
+}
+
+extern "C" int sdb_conv_wgrad_bf16_nd(const void* d_x, const void* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
+                                      int uz, int uy, int ux, int kz, int kyx, const void* d_dy, int dy_bf16, int ldy, int cout,
+                                      float* d_work, long long work_floats, float* d_dw, float* d_db, sdb_stream_t stream) {
+  if ((kz != 1 && kz != 3) || (kyx != 1 && kyx != 3) || (kz == 3 && kyx != 3)) { sdb::set_error("conv_wgrad_bf16_nd: kernel must be 1^d, 3^d or (1, 3, 3)"); return 1; }
+  return conv_wgrad("conv_wgrad_bf16_nd", d_x, d_x_lo, n, d, h, w, cin_skip, cin_lo, uz, uy, ux, kz, kyx, kyx, d_dy, ldy, cout, d_work,
+                    work_floats, d_dw, d_db, (cudaStream_t)stream, dy_bf16 ? sdb::WGRAD_BF16_DY_BF16 : sdb::WGRAD_BF16_DY_F32);
 }
 
 extern "C" int sdb_conv_wgrad_any_nd(const float* d_x, const float* d_x_lo, int n, int d, int h, int w, int cin_skip, int cin_lo,
@@ -531,14 +487,14 @@ extern "C" int sdb_decoder_split(const float* d_dcat, int n, int d, int h, int w
   cudaStream_t st = (cudaStream_t)stream;
   if (c_lo < 1 || c_skip < 1 || uz < 1 || uy < 1 || ux < 1 || d % uz || h % uy || w % ux) { sdb::set_error("decoder_split: bad arguments"); return 1; }
   const long long total = (long long)n * d * h * w / ((long long)uz * uy * ux) * c_lo + (long long)n * d * h * w * c_skip;
-  SDB_LAUNCH(k_decoder_split, grid_1d(total, 32), 256, 0, st, d_dcat, n, d, h, w, c_lo, c_skip, uz, uy, ux, d_dlo, d_dskip);
+  SDB_LAUNCH(sdb::k_decoder_split<float>, grid_1d(total, 32), 256, 0, st, d_dcat, n, d, h, w, c_lo, c_skip, uz, uy, ux, d_dlo, d_dskip);
   return 0;
 }
 
 extern "C" int sdb_relu_backward(float* d_g, const float* d_y, long long n, sdb_stream_t stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) return 0;
-  SDB_LAUNCH(k_relu_backward, grid_1d(n, 32), 256, 0, st, d_g, d_y, n);
+  SDB_LAUNCH(sdb::k_relu_backward<float>, grid_1d(n, 32), 256, 0, st, d_g, d_y, n);
   return 0;
 }
 
@@ -547,7 +503,7 @@ extern "C" int sdb_maxpool_backward_nd(const float* d_x, const float* d_gy, int 
   cudaStream_t st = (cudaStream_t)stream;
   if (pz < 1 || py < 1 || px < 1 || d % pz || h % py || w % px || c < 1) { sdb::set_error("maxpool_backward_nd: sizes must be divisible by the pool"); return 1; }
   const long long total = (long long)n * (d / pz) * (h / py) * (w / px) * c;
-  SDB_LAUNCH(k_maxpool_backward, grid_1d(total, 32), 256, 0, st, d_x, d_gy, n, d, h, w, c, pz, py, px, accumulate, d_gx);
+  SDB_LAUNCH(sdb::k_maxpool_backward<float>, grid_1d(total, 32), 256, 0, st, d_x, d_gy, n, d, h, w, c, pz, py, px, accumulate, d_gx);
   return 0;
 }
 

@@ -4,6 +4,8 @@ StarDist2D.train / StarDist3D.train.
 Reference: stardist/models/model2d.py:352-481 / model3d.py `train`, the losses of stardist/models/base.py:34-50,
 :108-126 (the multi-class cross-entropy) and :315-347, Keras' Adam, ReduceLROnPlateau and csbdeep's checkpointing
 (restated on the host below).  The forward pass is UNetDeviceND's (exact fp32 CUDA cores) with its activations kept; DESIGN.md 4.2 states the data flow and the loss.
+Under the 'mixed_bfloat16' policy of stardist_b200.mixed_precision the trainer runs its own forward pass and every
+convolution, head and gradient between layers on the bf16 tensor-core kernels of csrc/unet_train_bf16.cu instead.
 """
 import warnings
 import numpy as np
@@ -31,8 +33,9 @@ def tensor_float_32_execution_enabled():
     return _tensor_float_32
 
 
-def check_trainable(config, optimizer=None):
-    """NotImplementedError for every setting this trainer does not cover; runs before anything touches the device"""
+def check_trainable(config, optimizer=None, policy=None):
+    """NotImplementedError for every setting this trainer does not cover under `policy` (default: the global mixed-precision
+    policy); runs before anything touches the device"""
     if getattr(config, 'backbone', 'unet') != 'unet':
         raise NotImplementedError("training of the '%s' backbone is not supported (U-Net only)" % config.backbone)
     if config.train_dist_loss not in ('mae', 'mse'):
@@ -56,6 +59,23 @@ def check_trainable(config, optimizer=None):
         for l in unet_layers(config):
             if l['kind'] == 'conv_class' and l['cin'] % 32:
                 raise NotImplementedError("layer %s: %d input channels; the input gradient needs a multiple of 32" % (l['name'], l['cin']))
+    from ..mixed_precision import global_policy
+    if (global_policy() if policy is None else policy).name == 'mixed_bfloat16':
+        check_bf16(config)
+
+
+def check_bf16(config):
+    """NotImplementedError naming the first layer the mixed_bfloat16 kernels do not take (unet_device.conv_bf16_accepts)"""
+    from .unet_device import conv_bf16_accepts
+    from .weights import unet_layers
+    for l in unet_layers(config):
+        if l['kind'] in ('conv', 'conv_class'):
+            lo = l.get('cin_lo', 0)
+            if not conv_bf16_accepts(config.n_dim, l['k'], l['cin'] - lo, lo, l['cout'], l['act']):
+                raise NotImplementedError(
+                    "policy 'mixed_bfloat16': layer %s (kernel %s, %d -> %d channels, activation %r) is outside the bf16 family: "
+                    "kernels 1^d, 3^d or (1, 3, 3), ReLU or linear, output channels a multiple of 32, input channels <= 4 (stem) "
+                    "or a multiple of 8" % (l['name'], tuple(l['k']), l['cin'], l['cout'], l['act']))
 
 
 def adam_coef(n):
@@ -69,12 +89,17 @@ class UNetTrainer:
     """Device parameters (one flat float32 buffer), Adam's m and v, the forward activations and the backward buffers of
     one U-Net.  step() runs forward, loss, backward and Adam without reading anything back to the host."""
 
+    bf16 = False        # set from the mixed-precision policy at construction
+
     def __init__(self, config, weights, learning_rate=None):
         import torch
         from .unet_device import UNetDeviceND
-        check_trainable(config)
+        from ..mixed_precision import global_policy
+        self.policy = global_policy()
+        self.bf16 = self.policy.name == 'mixed_bfloat16'
+        check_trainable(config, policy=self.policy)
         lib = L.require_cuda()
-        self.tf32 = tensor_float_32_execution_enabled()
+        self.tf32 = tensor_float_32_execution_enabled() and not self.bf16
         self.config, self.nd = config, config.n_dim
         self.net = UNetDeviceND(config, weights)
         self.layers = self.net.layers
@@ -115,11 +140,12 @@ class UNetTrainer:
             self.class_w = torch.from_numpy(np.asarray(config.train_class_weights, np.float32)).to(dev)
 
     # ---------------------------------------------------------------------------------------------- buffers
-    def _buf(self, key, shape, zero=False):
+    def _buf(self, key, shape, zero=False, bf16=False):
         import torch
         b = self._bufs.get(key)
         if b is None or tuple(b.shape) != tuple(shape):
-            b = (torch.zeros if zero else torch.empty)(tuple(shape), dtype=torch.float32, device=self.net.device)
+            b = (torch.zeros if zero else torch.empty)(tuple(shape), dtype=torch.bfloat16 if bf16 else torch.float32,
+                                                       device=self.net.device)
             self._bufs[key] = b
         return b
 
@@ -144,7 +170,12 @@ class UNetTrainer:
         uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
         need = int(lib.sdb_conv_wgrad_workspace(n * d * h * w, kz * ky * kx, c_skip + c_lo, cout))
         work = self._workspace(need)
-        if conv_wgrad_accepts(self.nd, k):
+        if self.bf16:
+            import torch
+            L.check(lib.sdb_conv_wgrad_bf16_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, L.ptr(dy),
+                                               1 if dy.dtype == torch.bfloat16 else 0, ldy, cout, L.ptr(work), work.numel(), L.ptr(dw),
+                                               L.ptr(db), L.stream_ptr()))
+        elif conv_wgrad_accepts(self.nd, k):
             wgrad = lib.sdb_conv_wgrad_tf32_nd if self.tf32 else lib.sdb_conv_wgrad_nd
             L.check(wgrad(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, L.ptr(dy), ldy,
                           cout, L.ptr(work), work.numel(), L.ptr(dw), L.ptr(db), L.stream_ptr()))
@@ -184,6 +215,15 @@ class UNetTrainer:
         lib = L.load()
         st = L.stream_ptr()
         taps = int(np.prod(k))
+        if self.bf16:
+            kz, ky, kx = ((1,) + tuple(k)) if self.nd == 2 else tuple(k)
+            n = x_shape[0]; d, h, w = (1,) + tuple(x_shape[1:3]) if len(x_shape) == 4 else tuple(x_shape[1:4])
+            wfb = self._buf(('wflip_bf16', key), (taps * cout * cin,), bf16=True)
+            L.check(lib.sdb_weights_bf16(L.ptr(self.pview[name][0]), taps, cin, cout, 1, cout, L.ptr(wfb), st))
+            gin = self._buf(('gin', key), tuple(x_shape[:-1]) + (cin,), bf16=True)
+            L.check(lib.sdb_conv_bf16_nd(L.ptr(g), None, n, d, h, w, cout, 0, 1, 1, 1, kz, ky, kx, L.ptr(wfb), None, cin, 0, 0,
+                                         L.ptr(gin), st))
+            return gin
         wf = self._buf(('wflip', key), (taps, cout, cin))
         L.check(lib.sdb_conv_flip_weights(L.ptr(self.pview[name][0]), taps, cin, cout, L.ptr(wf), st))
         n = x_shape[0]; d, h, w = (1,) + tuple(x_shape[1:3]) if len(x_shape) == 4 else tuple(x_shape[1:4])
@@ -203,7 +243,9 @@ class UNetTrainer:
         """g *= act'(pre-activation) in place: from the output y for ReLU, from the kept pre-activation z for the activations
         other than ReLU / linear"""
         lib = L.load()
-        if act == 'relu':
+        if act == 'relu' and self.bf16:
+            L.check(lib.sdb_relu_backward_bf16(L.ptr(g), L.ptr(y), g.numel(), L.stream_ptr()))
+        elif act == 'relu':
             L.check(lib.sdb_relu_backward(L.ptr(g), L.ptr(y), g.numel(), L.stream_ptr()))
         elif act != 'linear':
             from .unet_device import act_id
@@ -221,13 +263,23 @@ class UNetTrainer:
         ones = (1,) * self.nd
         self._wgrad(xc, None, ones, ones, dclass, C, C, *self.gview['prob_class'])
         wc = self.pview['prob_class'][0]
+        if self.bf16:
+            wcb = self._buf('wclass_bwd_bf16', (cf * C,), bf16=True)
+            L.check(lib.sdb_weights_bf16(L.ptr(wc), 1, cf, C, 1, C, L.ptr(wcb), st))
         if 'features_class' not in self.pview:
-            L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 0, 1, L.ptr(g), st))
+            if self.bf16:
+                L.check(lib.sdb_gemm_bf16_f32in(L.ptr(dclass), npix, C, L.ptr(wcb), cf, 1, L.ptr(g), st))
+            else:
+                L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 0, 1, L.ptr(g), st))
             return None
-        gc = self._buf('dfeat_class', xc.shape)
+        gc = self._buf('dfeat_class', xc.shape, bf16=self.bf16)
         act = self.config.unet_activation
-        L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 1 if act == 'relu' else 0, 0, L.ptr(gc), st))
-        if act != 'relu':
+        if self.bf16:
+            L.check(lib.sdb_gemm_bf16_f32in(L.ptr(dclass), npix, C, L.ptr(wcb), cf, 0, L.ptr(gc), st))
+            self._act_backward(gc, act, xc, None)
+        else:
+            L.check(lib.sdb_class_head_backward(L.ptr(xc), L.ptr(dclass), npix, cf, L.ptr(wc), C, 1 if act == 'relu' else 0, 0, L.ptr(gc), st))
+        if act != 'relu' and not self.bf16:
             self._act_backward(gc, act, xc, self.net.saved_class_z)
         k = tuple(self.pview['features_class'][0].shape[:self.nd])
         self._wgrad(base, None, ones, k, gc, cf, cf, *self.gview['features_class'])
@@ -246,9 +298,15 @@ class UNetTrainer:
         dh = dhead.view(-1)
         self._wgrad(feat, None, ones, ones, dh, R + 1, 1, *self.gview['prob'])
         self._wgrad(feat, None, ones, ones, dh[1:], R + 1, R, *self.gview['dist'])
-        g = self._buf('dfeat', feat.shape)
-        L.check(lib.sdb_heads_backward(L.ptr(feat), L.ptr(dhead), npix, cf, L.ptr(self.pview['prob'][0]), L.ptr(self.pview['dist'][0]),
-                                       R, 0, L.ptr(g), st))
+        g = self._buf('dfeat', feat.shape, bf16=self.bf16)
+        if self.bf16:
+            whb = self._buf('wheads_bwd_bf16', (cf * (R + 1),), bf16=True)
+            L.check(lib.sdb_weights_bf16(L.ptr(self.pview['prob'][0]), 1, cf, 1, 1, R + 1, L.ptr(whb), st))
+            L.check(lib.sdb_weights_bf16(L.ptr(self.pview['dist'][0]), 1, cf, R, 1, R + 1, L.ptr(whb[1:]), st))
+            L.check(lib.sdb_gemm_bf16_f32in(L.ptr(dhead), npix, R + 1, L.ptr(whb), cf, 0, L.ptr(g), st))
+        else:
+            L.check(lib.sdb_heads_backward(L.ptr(feat), L.ptr(dhead), npix, cf, L.ptr(self.pview['prob'][0]), L.ptr(self.pview['dist'][0]),
+                                           R, 0, L.ptr(g), st))
         gin_class = None if dclass is None else self._class_backward(dclass, g)
         first = next(i for i, l in enumerate(self.layers) if l['kind'] == 'conv')
         skip_grad = {}
@@ -265,15 +323,18 @@ class UNetTrainer:
                 n = x.shape[0]; d, h, w = self._dhw(x)
                 gin = self._dgrad(i, l['name'], g, x.shape, l['cin'], cout, l['k'])
                 if gin_class is not None and l['name'] == 'features':
-                    L.check(lib.sdb_add_act(L.ptr(gin), L.ptr(gin_class), gin.numel(), 0, L.ptr(gin), st))
+                    if self.bf16:
+                        L.check(lib.sdb_add_bf16(L.ptr(gin), L.ptr(gin_class), gin.numel(), L.ptr(gin), st))
+                    else:
+                        L.check(lib.sdb_add_act(L.ptr(gin), L.ptr(gin_class), gin.numel(), 0, L.ptr(gin), st))
                 if lo is not None:
                     up_layer = self.layers[i - 1]
                     assert up_layer['kind'] == 'up'
                     uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
-                    dlo = self._buf(('dlo', i), lo.shape)
-                    dskip = self._buf(('dskip', i), x.shape)
-                    L.check(lib.sdb_decoder_split(L.ptr(gin), n, d, h, w, lo.shape[-1], x.shape[-1], int(uz), int(uy), int(ux),
-                                                  L.ptr(dlo), L.ptr(dskip), st))
+                    dlo = self._buf(('dlo', i), lo.shape, bf16=self.bf16)
+                    dskip = self._buf(('dskip', i), x.shape, bf16=self.bf16)
+                    split = lib.sdb_decoder_split_bf16 if self.bf16 else lib.sdb_decoder_split
+                    L.check(split(L.ptr(gin), n, d, h, w, lo.shape[-1], x.shape[-1], int(uz), int(uy), int(ux), L.ptr(dlo), L.ptr(dskip), st))
                     skip_grad[up_layer['skip']] = dskip
                     g = dlo
                 else:
@@ -285,19 +346,119 @@ class UNetTrainer:
                 if 'save_skip' in l:
                     gx, acc = skip_grad.pop(l['save_skip']), 1
                 else:
-                    gx, acc = self._buf(('gpool', i), x.shape), 0
-                L.check(lib.sdb_maxpool_backward_nd(L.ptr(x), L.ptr(g), n, d, h, w, x.shape[-1], int(pz), int(py), int(px), acc,
-                                                    L.ptr(gx), st))
+                    gx, acc = self._buf(('gpool', i), x.shape, bf16=self.bf16), 0
+                pool_bwd = lib.sdb_maxpool_backward_bf16_nd if self.bf16 else lib.sdb_maxpool_backward_nd
+                L.check(pool_bwd(L.ptr(x), L.ptr(g), n, d, h, w, x.shape[-1], int(pz), int(py), int(px), acc, L.ptr(gx), st))
                 g = gx
+
+    # ---------------------------------------------------------------------------------------------- mixed_bfloat16 forward
+    def _forward_bf16(self, x):
+        """the forward pass under 'mixed_bfloat16': the input rounded to bf16 once, every convolution on sdb_conv_bf16_nd with bf16
+        kernels copied from the fp32 parameters, bf16 max pooling, fp32 prob / dist / prob_class from bf16 features.  Keeps in
+        self.net what _backward reads, as UNetDeviceND.forward(keep=True) does, with bf16 tensors."""
+        import torch
+        lib = L.load()
+        st = L.stream_ptr()
+        net, nd = self.net, self.nd
+        ones = (1,) * nd
+        cur = self._buf('x_bf16', x.shape, bf16=True)
+        L.check(lib.sdb_cast_bf16(L.ptr(x), x.numel(), L.ptr(cur), st))
+        skips, saved = {}, [None] * len(self.layers)
+        lo, up, base = None, ones, None
+        for i, l in enumerate(self.layers):
+            kind = l['kind']
+            if kind == 'conv':
+                if l['name'] == 'features':
+                    base = cur
+                y = self._conv_bf16(cur, lo, up, l)
+                saved[i] = dict(x=cur, lo=lo, up=up, y=y, z=None)
+                cur, lo, up = y, None, ones
+            elif kind == 'pool':
+                if 'save_skip' in l:
+                    skips[l['save_skip']] = cur
+                saved[i] = dict(x=cur)
+                n = cur.shape[0]; d, h, w = self._dhw(cur); c = cur.shape[-1]
+                pz, py, px = ((1,) + tuple(l['pool'])) if nd == 2 else tuple(l['pool'])
+                osp = (h // py, w // px) if nd == 2 else (d // pz, h // py, w // px)
+                out = torch.empty((n,) + osp + (c,), dtype=torch.bfloat16, device=cur.device)
+                L.check(lib.sdb_maxpool_bf16_nd(L.ptr(cur), n, d, h, w, c, int(pz), int(py), int(px), L.ptr(out), st))
+                cur = out
+            elif kind == 'up':
+                lo, up = cur, tuple(l['pool'])
+                cur = skips.pop(l['skip'])
+            elif kind == 'head':
+                break
+        feat = cur
+        net.saved, net.saved_feat = saved, feat
+        R, cf = self.config.n_rays, feat.shape[-1]
+        npix = feat.numel() // cf
+        whb = self._buf('wheads_bf16', ((R + 1) * cf,), bf16=True)
+        L.check(lib.sdb_weights_bf16(L.ptr(self.pview['prob'][0]), 1, cf, 1, 0, cf, L.ptr(whb), st))
+        L.check(lib.sdb_weights_bf16(L.ptr(self.pview['dist'][0]), 1, cf, R, 0, cf, L.ptr(whb[cf:]), st))
+        prob = torch.empty(tuple(feat.shape[:-1]), dtype=torch.float32, device=feat.device)
+        dist = torch.empty(tuple(feat.shape[:-1]) + (R,), dtype=torch.float32, device=feat.device)
+        L.check(lib.sdb_heads_bf16(L.ptr(feat), npix, cf, L.ptr(whb), L.ptr(self.pview['prob'][1]), L.ptr(self.pview['dist'][1]), R,
+                                   L.ptr(prob), L.ptr(dist), st))
+        net.prob_class = None
+        if self.n_classes is not None:
+            base = feat if base is None else base
+            xc = base
+            if 'features_class' in self.pview:
+                fl = next(l for l in self.layers if l['name'] == 'features_class')
+                xc = self._conv_bf16(base, None, ones, fl)
+            C = self.n_classes + 1
+            wcb = self._buf('wclass_bf16', (C * xc.shape[-1],), bf16=True)
+            L.check(lib.sdb_weights_bf16(L.ptr(self.pview['prob_class'][0]), 1, xc.shape[-1], C, 0, xc.shape[-1], L.ptr(wcb), st))
+            logits = self._buf('class_logits', tuple(xc.shape[:-1]) + (C,))
+            out = torch.empty(tuple(xc.shape[:-1]) + (C,), dtype=torch.float32, device=xc.device)
+            L.check(lib.sdb_class_head_bf16(L.ptr(xc), npix, xc.shape[-1], L.ptr(wcb), L.ptr(self.pview['prob_class'][1]), C,
+                                            L.ptr(logits), L.ptr(out), st))
+            net.saved_class, net.saved_class_z, net.prob_class = (base, xc, out), None, out
+        return prob, dist
+
+    def _conv_bf16(self, x, lo, up, l):
+        """act(conv([upsample(lo), x]) + bias) of layer l as bf16, from a bf16 copy of its fp32 kernel"""
+        import torch
+        lib = L.load()
+        st = L.stream_ptr()
+        name, cout = l['name'], l['cout']
+        k = tuple(l['k'])
+        taps = int(np.prod(k))
+        n = x.shape[0]; d, h, w = self._dhw(x)
+        c_skip, c_lo = x.shape[-1], 0 if lo is None else lo.shape[-1]
+        cin = c_skip + c_lo
+        wb = self._buf(('wb', name), (taps * cout * cin,), bf16=True)
+        L.check(lib.sdb_weights_bf16(L.ptr(self.pview[name][0]), taps, cin, cout, 0, cin, L.ptr(wb), st))
+        kz, ky, kx = ((1,) + k) if self.nd == 2 else k
+        uz, uy, ux = ((1,) + tuple(up)) if len(up) == 2 else tuple(up)
+        y = torch.empty(tuple(x.shape[:-1]) + (cout,), dtype=torch.bfloat16, device=x.device)
+        L.check(lib.sdb_conv_bf16_nd(L.ptr(x), L.ptr(lo), n, d, h, w, c_skip, c_lo, int(uz), int(uy), int(ux), kz, ky, kx, L.ptr(wb),
+                                     L.ptr(self.pview[name][1]), cout, 1 if l['act'] == 'relu' else 0, 0, L.ptr(y), st))
+        return y
 
     # ---------------------------------------------------------------------------------------------- public
     def _forward_loss(self, x, prob_t, dam, dhead, out, state, prob_class_t=None, dclass=None):
         import torch
         x = x if x.is_contiguous() else x.contiguous()
-        prob, dist = self.net.forward(x, keep=dhead is not None)
+        if self.bf16:
+            prob, dist = self._forward_bf16(x)
+        else:
+            prob, dist = self.net.forward(x, keep=dhead is not None)
         self._loss(prob, dist, prob_t, dam, dhead, out, state)
         if self.n_classes is not None:
             self._class_loss(self.net.prob_class, prob_class_t, dclass, out)
+
+    def saved_activations(self):
+        """the distinct device tensors the last forward pass kept for the backward pass"""
+        net, seen, out = self.net, set(), []
+        ts = [v for a in net.saved if a is not None for v in a.values() if hasattr(v, 'data_ptr')] + [net.saved_feat]
+        if self.n_classes is not None:
+            ts += list(net.saved_class[:2])            # the third entry is the fp32 prob_class output
+        for t in ts:
+            if t is not None and t.data_ptr() not in seen:
+                seen.add(t.data_ptr())
+                out.append(t)
+        return out
 
     def _n_out(self):
         return 4 if self.n_classes is None else 5

@@ -78,6 +78,17 @@ def conv_dgrad3_accepts(nd, k, cin, cout):
     return conv3_accepts(nd, k, (1,) * nd, cout, 0, cin, 'linear')
 
 
+def conv_bf16_accepts(nd, k, cin_skip, cin_lo, cout, act):
+    """the convolutions the mixed_bfloat16 trainer runs (csrc/unet_train_bf16.cu): kernels 1^d, 3^d and (1, 3, 3) in 3-D at
+    stride 1, ReLU or linear, cout a multiple of 32, and either the stem (cin <= 4 without an up-sampled source) or input
+    channels in multiples of 8, with or without the decoder's [upsample(lo), skip] input"""
+    if not conv_wgrad_accepts(nd, k) or act not in ('relu', 'linear') or cout % 32:
+        return False
+    if cin_lo == 0 and 1 <= cin_skip <= 4:
+        return True
+    return cin_skip > 0 and cin_skip % 8 == 0 and cin_lo % 8 == 0
+
+
 def keeps_preactivation(act):
     """training keeps the pre-activation z of layers whose activation derivative needs it (every activation but ReLU and
     linear, whose backward reads the output)"""
