@@ -583,6 +583,13 @@ int sdb_stardist_class_loss(const float* d_s, const float* d_t, long long npix, 
  * to d_dfeat instead of overwriting it */
 int sdb_class_head_backward(const float* d_feat, const float* d_dz, long long npix, int cfeat, const float* d_w, int n_out,
                             int relu, int accumulate, float* d_dfeat, sdb_stream_t stream);
+/* Data-parallel reduction of one training step (DESIGN.md 4.2).  d_rows [world][ld]: replica r's flat gradient in
+ * d_rows[r * ld, + n_params) followed by its loss row (loss, prob_loss, dist_loss, skipped[, prob_class_loss]) of n_out >= 4
+ * floats.  S = the replicas with skipped == 0 in ascending rank order, all replicas when none is.  Writes d_g = (sum over S) / |S|
+ * and d_out [n_out] likewise (fp32 additions from S's first member, then one fp32 division), and advances the step state
+ * d_state = (t, n_skipped, skip) once, skipped when no replica is.  d_rows and d_g may alias for world = 1.  No atomics. */
+int sdb_replica_reduce(const float* d_rows, int world, long long n_params, int n_out, long long ld, float* d_g, float* d_out,
+                       int* d_state, sdb_stream_t stream);
 /* TF2 Keras Adam over n parameters; alpha = lr * coef[t - 1] with t = d_state[0]; nothing when d_state[2] (skipped step) */
 int sdb_adam_step(float* d_w, const float* d_g, float* d_m, float* d_v, long long n, float lr, float one_minus_b1,
                   float one_minus_b2, float eps, const float* d_coef, const int* d_state, sdb_stream_t stream);

@@ -129,6 +129,8 @@ def _declare(lib):
     lib.sdb_class_head_backward.restype = c_int
     lib.sdb_adam_step.argtypes = [P, P, P, P, c_longlong, c_float, c_float, c_float, c_float, P, P, P]
     lib.sdb_adam_step.restype = c_int
+    lib.sdb_replica_reduce.argtypes = [P, c_int, c_longlong, c_int, c_longlong, P, P, P, P]
+    lib.sdb_replica_reduce.restype = c_int
     lib.sdb_heads_2d.argtypes = [P, c_longlong, c_int, P, P, P, P, c_int, P, P, P]
     lib.sdb_conv3x3_tc.argtypes = [P, P, c_int, P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, c_int, P, P, P]
     lib.sdb_heads_tc.argtypes = [P, P, c_int, c_int, c_int, c_int, P, P, c_float, P, c_int, c_int, P, P, P]

@@ -1,6 +1,7 @@
 // unet_train.cu -- fp32 CUDA-core kernels of the U-Net training step (NHWC / NDHWC): weight gradients of the
 // 3^d / 1^d convolutions, the decoder split, ReLU and max-pool backward (the float instances of train_elem.cuh), the StarDist loss with its head gradient,
-// the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients and Adam.  The input gradient of the
+// the multi-class cross-entropy with its softmax-logit gradient, the 1x1 head input gradients, the data-parallel reduction of the
+// replicas' gradients and Adam.  The input gradient of the
 // convolutions is not here: it is a forward kernel run on dY with the spatially flipped, Cin/Cout-transposed kernel written by
 // sdb_conv_flip_weights -- sdb_conv3_nd of unet_simt.cu for the 3^d layers it takes, sdb_conv_dgrad_any_nd of unet_any.cu
 // for every other kernel extent and channel count.
@@ -11,6 +12,7 @@
 #include <math.h>
 #include <string>
 #include <algorithm>
+#include <cstdint>
 #include "common.cuh"
 #include "wgrad.cuh"
 #include "train_elem.cuh"
@@ -395,6 +397,60 @@ __global__ void k_adam(float* __restrict__ w, const float* __restrict__ g, float
 
 int grid_1d(long long n, int per) { return (int)std::max<long long>(1, std::min<long long>(cdiv(n, 256), 132LL * per)); }
 
+// ------------------------------------------------------------------------------------------ data-parallel reduction
+constexpr int REDUCE_WORLD_MAX = 4096;   // the member list lives in shared memory
+// rows [W][ld]: replica r's flat gradient in rows[r * ld, + P) and its loss row (loss, prob_loss, dist_loss, skipped[, ...]) in
+// rows[r * ld + P, + n_out).  S = the replicas with skipped == 0 in ascending rank order, or all W replicas when none is: g[i] =
+// (S_0[i] + S_1[i] + ...) / |S| and out[k] likewise, fp32 additions from the first member, then one fp32 division.  Block 0 also
+// advances the shared step state as k_loss_final does for one batch, with skip = (no replica ok).  rows and g may alias (W = 1:
+// every element is read by the thread that writes it), so neither is __restrict__.  vec = 1: ld % 4 == 0 and 16-byte aligned
+// rows and g, read and written as float4 up to P rounded down to 4.
+__global__ void __launch_bounds__(256) k_replica_reduce(const float* rows, int W, long long P, int n_out, long long ld, int vec, float* g,
+                                                        float* __restrict__ out, int* __restrict__ state) {
+  extern __shared__ int sel[];             // [W]: the members of S, then their count in sel[W]
+  if (threadIdx.x == 0) {
+    int n = 0;
+    for (int r = 0; r < W; ++r)
+      if (rows[(size_t)r * ld + P + 3] == 0.f) sel[n++] = r;
+    const int skip = n == 0;
+    if (skip)
+      for (int r = 0; r < W; ++r) sel[n++] = r;
+    sel[W] = n;
+    if (blockIdx.x == 0) {
+      for (int k = 0; k < n_out; ++k) {
+        float a = rows[(size_t)sel[0] * ld + P + k];
+        for (int j = 1; j < n; ++j) a = __fadd_rn(a, rows[(size_t)sel[j] * ld + P + k]);
+        out[k] = __fdiv_rn(a, (float)n);
+      }
+      state[2] = skip;
+      if (skip) state[1] += 1; else state[0] += 1;
+    }
+  }
+  __syncthreads();
+  const int n = sel[W];
+  const float fn = (float)n;
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+  long long done = 0;
+  if (vec) {
+    const long long P4 = P / 4;
+    for (long long e = tid; e < P4; e += stride) {
+      float4 a = reinterpret_cast<const float4*>(rows + (size_t)sel[0] * ld)[e];
+      for (int j = 1; j < n; ++j) {
+        const float4 b = reinterpret_cast<const float4*>(rows + (size_t)sel[j] * ld)[e];
+        a.x = __fadd_rn(a.x, b.x); a.y = __fadd_rn(a.y, b.y); a.z = __fadd_rn(a.z, b.z); a.w = __fadd_rn(a.w, b.w);
+      }
+      a.x = __fdiv_rn(a.x, fn); a.y = __fdiv_rn(a.y, fn); a.z = __fdiv_rn(a.z, fn); a.w = __fdiv_rn(a.w, fn);
+      reinterpret_cast<float4*>(g)[e] = a;
+    }
+    done = P4 * 4;
+  }
+  for (long long e = done + tid; e < P; e += stride) {
+    float a = rows[(size_t)sel[0] * ld + e];
+    for (int j = 1; j < n; ++j) a = __fadd_rn(a, rows[(size_t)sel[j] * ld + e]);
+    g[e] = __fdiv_rn(a, fn);
+  }
+}
+
 }  // namespace
 
 extern "C" long long sdb_conv_wgrad_workspace(long long npix, int taps, int cin, int cout) {
@@ -572,5 +628,19 @@ extern "C" int sdb_adam_step(float* d_w, const float* d_g, float* d_m, float* d_
   cudaStream_t st = (cudaStream_t)stream;
   if (n <= 0) return 0;
   SDB_LAUNCH(k_adam, grid_1d(n, 8), 256, 0, st, d_w, d_g, d_m, d_v, n, lr, one_minus_b1, one_minus_b2, eps, d_coef, d_state);
+  return 0;
+}
+
+extern "C" int sdb_replica_reduce(const float* d_rows, int world, long long n_params, int n_out, long long ld, float* d_g, float* d_out,
+                                  int* d_state, sdb_stream_t stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  if (world < 1 || world > REDUCE_WORLD_MAX || n_params < 0 || n_out < 4 || ld < n_params + n_out) {
+    sdb::set_error("replica_reduce: 1 <= world <= 4096, n_out >= 4 and ld >= n_params + n_out required");
+    return 1;
+  }
+  const int vec = ld % 4 == 0 && (uintptr_t)d_rows % 16 == 0 && (uintptr_t)d_g % 16 == 0;
+  const long long work = vec ? std::max(n_params / 4, n_params % 4) : n_params;
+  SDB_LAUNCH(k_replica_reduce, grid_1d(work, 8), 256, (size_t)(world + 1) * sizeof(int), st, d_rows, world, n_params, n_out, ld, vec,
+             d_g, d_out, d_state);
   return 0;
 }

@@ -6,6 +6,7 @@ Reference: stardist/models/model2d.py:352-481 / model3d.py `train`, the losses o
 (restated on the host below).  The forward pass is UNetDeviceND's (exact fp32 CUDA cores) with its activations kept; DESIGN.md 4.2 states the data flow and the loss.
 Under the 'mixed_bfloat16' policy of stardist_b200.mixed_precision the trainer runs its own forward pass and every
 convolution, head and gradient between layers on the bf16 tensor-core kernels of csrc/unet_train_bf16.cu instead.
+With an initialised torch.distributed group, train() is data-parallel over its ranks (UNetTrainer.step_replica; DESIGN.md 4.2).
 """
 import warnings
 import numpy as np
@@ -118,7 +119,10 @@ class UNetTrainer:
         total = off
         dev = self.net.device
         self.params = (torch.zeros if self.n_classes is not None else torch.empty)(total, dtype=torch.float32, device=dev)
-        self.grad = torch.zeros(total, dtype=torch.float32, device=dev)
+        # the gradient is the head of this replica's row for data-parallel steps: [grad | loss row | pad to 4 floats]
+        self.row_ld = -(-(total + self._n_out()) // 4) * 4
+        self.row = torch.zeros(self.row_ld, dtype=torch.float32, device=dev)
+        self.grad = self.row[:total]
         self.m = torch.zeros(total, dtype=torch.float32, device=dev)
         self.v = torch.zeros(total, dtype=torch.float32, device=dev)
         self.pview, self.gview = {}, {}
@@ -475,22 +479,77 @@ class UNetTrainer:
         """one training step on a batch (CUDA tensors as StarDistData*.batch_device gives them; prob_class_t for multi-class
         models); returns the device float32 [4] (loss, prob_loss, dist_loss, skipped) or, for multi-class models, [5] (loss,
         prob_loss, dist_loss, skipped, prob_class_loss) -- or writes it into `out`"""
-        import torch
-        lib = L.load()
         dclass = self._dclass(prob_class_t)
-        if self.n_calls + 1 > self.coef.numel():
-            self.coef = torch.from_numpy(adam_coef(max(1024, 2 * (self.n_calls + 1)))).to(self.net.device)
         self.n_calls += 1
         out = self._buf('out', (self._n_out(),)) if out is None else out
         npix = prob_t.numel()
         dhead = self._buf('dhead', (npix, self.config.n_rays + 1))
         self._forward_loss(x, prob_t, dam, dhead, out, self.state, prob_class_t, dclass)
         self._backward(dhead, dclass)
+        self._adam()
+        return out
+
+    def _adam(self):
+        import torch
+        lib = L.load()
+        if self.n_calls > self.coef.numel():
+            self.coef = torch.from_numpy(adam_coef(max(1024, 2 * self.n_calls))).to(self.net.device)
         one = np.float32(1)
         L.check(lib.sdb_adam_step(L.ptr(self.params), L.ptr(self.grad), L.ptr(self.m), L.ptr(self.v), self.params.numel(),
                                   float(self.lr), float(one - np.float32(ADAM_BETA_1)), float(one - np.float32(ADAM_BETA_2)),
                                   float(np.float32(ADAM_EPSILON)), L.ptr(self.coef), L.ptr(self.state), L.stream_ptr()))
+
+    def step_replica(self, x, prob_t, dam, prob_class_t=None, out=None):
+        """one data-parallel training step over the ranks of the initialised torch.distributed default group (a world of 1
+        without one): x and the targets are this rank's contiguous share of the global batch.  Forward, loss and backward write
+        this rank's row (its gradient, then its loss row, without touching the step state); the rows of all ranks are
+        gathered in rank order and sdb_replica_reduce writes their mean over the replicas with a labelled pixel into self.grad,
+        the mean loss row into `out` and the shared step state; Adam then runs as in step().  Every rank computes the same bits.
+        Returns `out` (as step() does)."""
+        lib = L.load()
+        dclass = self._dclass(prob_class_t)
+        self.n_calls += 1
+        n_out, P = self._n_out(), self.grad.numel()
+        out = self._buf('out', (n_out,)) if out is None else out
+        dhead = self._buf('dhead', (prob_t.numel(), self.config.n_rays + 1))
+        self._forward_loss(x, prob_t, dam, dhead, self.row[P:P + n_out], None, prob_class_t, dclass)
+        self._backward(dhead, dclass)
+        rows, world = self._gather_rows()
+        L.check(lib.sdb_replica_reduce(L.ptr(rows), world, P, n_out, self.row_ld, L.ptr(self.grad), L.ptr(out), L.ptr(self.state),
+                                       L.stream_ptr()))
+        self._adam()
         return out
+
+    def _gather_rows(self):
+        """(the [world][row_ld] rows of every rank in rank order, world): one all_gather over the default group, device to
+        device for NCCL, staged through host memory otherwise (gloo); this rank's own row for a world of 1"""
+        import torch
+        import torch.distributed as dist
+        from ..parallel_big import rank_world
+        _, world = rank_world()
+        if world == 1:
+            return self.row, 1
+        rows = self._buf('rows', (world, self.row_ld))
+        if 'nccl' in str(dist.get_backend()):
+            dist.all_gather_into_tensor(rows, self.row)
+        else:
+            host = torch.empty((world, self.row_ld), dtype=torch.float32)
+            dist.all_gather(list(host.unbind(0)), self.row.cpu())
+            rows.copy_(host)
+        return rows, world
+
+    def broadcast_params(self):
+        """make every rank's parameters rank 0's (the default group; nothing without one)"""
+        import torch.distributed as dist
+        from ..parallel_big import rank_world
+        if rank_world()[1] == 1:
+            return
+        if 'nccl' in str(dist.get_backend()):
+            dist.broadcast(self.params, 0)
+        else:
+            host = self.params.cpu()
+            dist.broadcast(host, 0)
+            self.params.copy_(host)
 
     def evaluate(self, x, prob_t, dam, prob_class_t=None):
         """forward pass and loss only: device float32 [4] (loss, prob_loss, dist_loss, n_p == 0), [5] with prob_class_loss
@@ -583,6 +642,14 @@ def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=Non
     validation_data's X, Y may be lazy sequences; they go to the generators as given, and the validation patches are made once."""
     config = model.config
     check_trainable(config, optimizer)
+    from ..parallel_big import rank_world
+    rank, world = rank_world()
+    import torch.distributed as dist
+    parallel = dist.is_available() and dist.is_initialized()
+    bs = int(config.train_batch_size)
+    if parallel and bs % world:
+        raise ValueError("train_batch_size = %d is the global batch of data-parallel training and must be divisible by the "
+                         "world size %d" % (bs, world))
     multi = config.n_classes is not None
     if multi:
         classes = model._parse_classes_arg(classes, len(X))
@@ -590,6 +657,8 @@ def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=Non
         warnings.warn("Ignoring given classes as n_classes is set to None")
     if seed is not None:
         np.random.seed(seed)
+    if parallel:
+        broadcast_random_state()
     if epochs is None:
         epochs = config.train_epochs
     if steps_per_epoch is None:
@@ -632,10 +701,13 @@ def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=Non
         model.data_train = Data(X, Y, batch_size=config.train_batch_size, augmenter=augmenter, length=epochs * steps_per_epoch, **kw)
 
     trainer = UNetTrainer(config, model.weights)
+    if parallel:
+        trainer.broadcast_params()
     rlr = ReduceLROnPlateau(**config.train_reduce_lr) if config.train_reduce_lr is not None else None
     best_ckpt = BestCheckpoint()
     logdir = getattr(model, 'logdir', None)
-    if logdir is not None:
+    write = logdir is not None and rank == 0           # with a group, rank 0 alone writes the model folder
+    if write:
         logdir.mkdir(parents=True, exist_ok=True)
         with open(logdir / 'config.json', 'w') as f:
             f.write(config.to_json())
@@ -644,27 +716,37 @@ def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=Non
     log = torch.empty((steps_per_epoch, 5 if multi else 4), dtype=torch.float32, device=trainer.net.device)
     cols = [0, 1, 2, 4] if multi else [0, 1, 2]
     names = [k for k in hist.history if k != 'lr']
-    bs = int(config.train_batch_size)
+    mine = slice(rank * (bs // world), (rank + 1) * (bs // world))       # this rank's items of the global batch
     best_weights = None
     for epoch in range(epochs):
         for s in range(steps_per_epoch):
             (x,), targets = model.data_train.batch_device(epoch * steps_per_epoch + s)
-            trainer.step(x, *targets, out=log[s])
-        # validation over batches of train_batch_size, weighted by batch size (Keras' evaluate)
-        vals = []
-        for b0 in range(0, n_take, bs):
-            b1 = min(n_take, b0 + bs)
-            vt = (cv[b0:b1],) if multi else ()
-            vals.append((b1 - b0, trainer.evaluate(xv[b0:b1], pv[b0:b1], dv[b0:b1], *vt)))
+            if parallel:
+                trainer.step_replica(x[mine], *(t[mine] for t in targets), out=log[s])
+            else:
+                trainer.step(x, *targets, out=log[s])
         steps = log.cpu().numpy()
-        vrows = np.stack([v.cpu().numpy() for _, v in vals])
-        vw = np.array([n for n, _ in vals], np.float64)
+        # validation over batches of train_batch_size, weighted by batch size (Keras' evaluate); with a group on rank 0, which
+        # then sends the result to every rank
+        va = None
+        if rank == 0:
+            vals = []
+            for b0 in range(0, n_take, bs):
+                b1 = min(n_take, b0 + bs)
+                vt = (cv[b0:b1],) if multi else ()
+                vals.append((b1 - b0, trainer.evaluate(xv[b0:b1], pv[b0:b1], dv[b0:b1], *vt)))
+            vrows = np.stack([v.cpu().numpy() for _, v in vals])
+            vw = np.array([n for n, _ in vals], np.float64)
+            va = (vrows[:, cols].astype(np.float64) * vw[:, None]).sum(axis=0) / vw.sum()
+        if parallel:
+            box = [va]
+            dist.broadcast_object_list(box, src=0)
+            va = box[0]
         ok = steps[:, 3] == 0
         if not ok.all():
             warnings.warn("epoch %d: %d training batch(es) without any labelled pixel (all prob targets < 0) were skipped"
                           % (epoch + 1, int((~ok).sum())))
         tr = steps[ok][:, cols].astype(np.float64).mean(axis=0) if ok.any() else np.full(len(cols), np.nan)
-        va = (vrows[:, cols].astype(np.float64) * vw[:, None]).sum(axis=0) / vw.sum()
         for k, v in zip(names, list(tr) + list(va)):
             hist.history[k].append(float(v))
         hist.history['lr'].append(float(trainer.lr))
@@ -673,15 +755,24 @@ def train(model, X, Y, validation_data, classes='auto', augmenter=None, seed=Non
             trainer.lr = rlr.on_epoch_end(va[0], trainer.lr)
         if best_ckpt.improved(va[0]):
             best_weights = trainer.weights()
-            if logdir is not None:
+            if write:
                 _save_weights(logdir / 'weights.npz', best_weights)
-        if logdir is not None:
+        if write:
             _save_weights(logdir / 'weights_last.npz', trainer.weights())
     # csbdeep's _training_finished: with a model folder the best checkpoint is loaded, otherwise the last weights stay
     final = trainer.weights()
     model.weights = best_weights if (logdir is not None and best_weights is not None) else final
     model._net = None
     return hist
+
+
+def broadcast_random_state():
+    """give every rank of the default group rank 0's numpy global random state, so that all ranks draw the same batches,
+    augmentations and validation patches"""
+    import torch.distributed as dist
+    box = [np.random.get_state()]
+    dist.broadcast_object_list(box, src=0)
+    np.random.set_state(box[0])
 
 
 def _save_weights(path, weights):
